@@ -1,3 +1,3 @@
-/* forwards the reference header name to the B200 host layer (see INTEGRATION.md section 2) */
+/* forwards the reference header name to the host layer of libmplb (see INTEGRATION.md section 2) */
 #pragma once
 #include <mpl_b200/traj_solver.hpp>

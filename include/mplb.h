@@ -1,5 +1,5 @@
 /*
- * mplb.h — C ABI of the B200-native motion-primitive lattice planner (libmplb.so).
+ * mplb.h — C ABI of the H100-native motion-primitive lattice planner (libmplb.so).
  *
  * This is the drop-in boundary for ONE path of sikang/mpl_ros: the A* wavefront
  *   PlannerBase::plan -> GraphSearch::Astar -> env_map::get_succ -> Primitive -> traverse_primitive -> MapUtil
@@ -13,7 +13,7 @@
  * (MPLB_OK = 0) unless noted; nothing is printed unless the planner was created verbose.  A planner handle
  * is not re-entrant (like the reference's PlannerBase, env_base.h:402-404); distinct planners may share one
  * map as long as nobody mutates it.  There is NO CPU fallback: every call that needs the device fails with
- * MPLB_ERR_CUDA when no CUDA device / sm_100 kernel image is usable.
+ * MPLB_ERR_CUDA when no CUDA device / sm_90 kernel image is usable.
  */
 #ifndef MPLB_H
 #define MPLB_H

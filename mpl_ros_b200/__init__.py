@@ -1,8 +1,8 @@
-"""mpl_ros_b200 — B200-native drop-in for the A* hot path of sikang/mpl_ros.
+"""mpl_ros_b200 — H100-native drop-in for the A* hot path of sikang/mpl_ros.
 
 Public surface (mirrors the reference's class names, see planner.py): MapUtil / OccMapUtil / VoxelMapUtil,
 Waypoint, Primitive, Trajectory, MapPlanner / OccMapPlanner / VoxelMapPlanner.  The compute lives in
-libmplb.so (hand-written sm_100a CUDA behind the C ABI of include/mplb.h); importing this package does not
+libmplb.so (hand-written sm_90a CUDA behind the C ABI of include/mplb.h); importing this package does not
 load it, the first call does, and it raises if the library or a CUDA device is missing.
 """
 from . import maps  # noqa: F401

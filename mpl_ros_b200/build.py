@@ -1,4 +1,4 @@
-"""In-tree build of libmplb.so for sm_100a (nvcc cross-compiles without a GPU).
+"""In-tree build of libmplb.so for sm_90a (H100; nvcc cross-compiles without a GPU).
 
 One object per translation unit (kept next to the sources, git-ignored), linked into mpl_ros_b200/libmplb.so; a unit is
 recompiled only when it or one of its headers is newer than its object."""
@@ -20,7 +20,7 @@ OUT = os.path.join(HERE, "libmplb.so")
 
 # -fmad=false: the reference is built without FMA contraction (MPL/CMakeLists.txt:5-8); the kernels also use
 # explicit __d*_rn intrinsics, the flag covers whatever remains.
-ARCH_FLAGS = ["-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-fmad=false"]
+ARCH_FLAGS = ["-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-fmad=false"]
 NVCC_FLAGS = ["-shared", "-Xcompiler", "-fPIC"] + ARCH_FLAGS
 
 

@@ -3,7 +3,7 @@
  *
  * Host side of the drop-in boundary: map objects (MapUtil, map_util.h), planner objects
  * (PlannerBase / MapPlanner, planner_base.h, map_planner.cpp:6-18), batch orchestration over arena tiers,
- * and result getters.  All compute runs in the sm_100a kernels of mplb_search.cuh; there is no CPU path.
+ * and result getters.  All compute runs in the sm_90a kernels of mplb_search.cuh; there is no CPU path.
  */
 #include <cuda_runtime.h>
 #include <dlfcn.h>
@@ -874,7 +874,7 @@ int run_batch_begin(mplb_planner *p, const mplb_waypoint *d_starts, const mplb_w
   }
   const int resident = p->resident_cached;
   if (p->sm_count == 0) cudaDeviceGetAttribute(&p->sm_count, cudaDevAttrMultiProcessorCount, p->device);
-  if (resident <= 0) return fail(MPLB_ERR_CUDA, "no resident CTA for the search kernel (is this an sm_100 device?)");
+  if (resident <= 0) return fail(MPLB_ERR_CUDA, "no resident CTA for the search kernel (is this an sm_90 device?)");
 
   if (p->budget_bytes == 0) {
     size_t free_b = 0, total_b = 0;

@@ -1,5 +1,5 @@
 /*
- * mplb_device.cuh — device-side arithmetic of the lattice planner (sm_100a).
+ * mplb_device.cuh — device-side arithmetic of the lattice planner (sm_90a).
  *
  * Every floating-point operation that the reference performs on the hot path is written here with
  * explicit round-to-nearest intrinsics (__dadd_rn / __dmul_rn / __ddiv_rn never contract to FMA), in the
@@ -23,12 +23,11 @@ namespace mplb {
 #endif
 #define MPLB_MAXU 128 /* max |U| */
 #ifndef MPLB_MIN_CTAS
-#define MPLB_MIN_CTAS 6 /* resident CTAs per SM the plain |U| <= 32 search kernel is compiled for.  Measured on the 65 536-query bench
-                           list (profiles/r02_cta_shape_sweep.md, prim/s x 1e9, threads x CTAs/SM): 256x3 2.41, 224x4 2.72, 192x5 2.60,
-                           256x4 2.62, 160x6 2.92, 128x8 2.78; with a 1-slot probe window 224x4 2.88, 192x5 2.77, 160x6 3.07,
-                           128x8 2.99.  More, smaller plans per SM hide the per-pop latency chain better than more sampling warps
-                           per plan once the batch is deep enough to keep every slot busy (a 1024-query batch is tail bound and
-                           prefers 256x3: 1.62 vs 1.29 for 192x5). */
+#define MPLB_MIN_CTAS 6 /* resident CTAs per SM the plain |U| <= 32 search kernel is compiled for (64 registers per thread of the
+                           64 K an SM has).  A sweep of threads x CTAs/SM on the 65 536-query bench list (256x3, 224x4, 192x5,
+                           256x4, 160x6, 128x8) put 160x6 first: more, smaller plans per SM hide the per-pop latency chain better
+                           than more sampling warps per plan once the batch is deep enough to keep every slot busy (a 1024-query
+                           batch is tail bound and prefers 256x3). */
 #endif
 
 __device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a, b); }
@@ -36,7 +35,7 @@ __device__ __forceinline__ double dsub(double a, double b) { return __dsub_rn(a,
 __device__ __forceinline__ double dmul(double a, double b) { return __dmul_rn(a, b); }
 __device__ __forceinline__ double ddiv(double a, double b) { return __ddiv_rn(a, b); }
 
-/* Rounding without the XU pipe.  On B200 every FP64 conversion / rounding instruction (F2I, I2F, FRND, MUFU.RCP64H)
+/* Rounding without the XU pipe.  Every FP64 conversion / rounding instruction (F2I, I2F, FRND, MUFU.RCP64H)
  * issues to the low-rate XU pipe and has a long latency on the serial chain of a pop; adding and subtracting
  * 1.5 * 2^52 rounds to nearest-even on the FP64 pipe instead and leaves the integer in the low mantissa word.
  * Valid for |x| < 2^31; used only inside filters that defer to the exact formula near ties. */

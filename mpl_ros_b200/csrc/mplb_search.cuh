@@ -10,8 +10,8 @@
  *                                 boost::heap::d_ary_heap<arity<2>, mutable_<true>> so pop order is identical)
  *   recoverTraj                   graph_search.h:369-455 (best-predecessor rule kept as a running argmin)
  *
- * The search of one plan is a serial chain of pops, so the kernel is latency-bound per plan (measured on B200:
- * dependent FP64 op 8.3 cycles, __ddiv_rn 125, LDS 34, SHFL 26, HBM round trip ~1000) and throughput comes from
+ * The search of one plan is a serial chain of pops, so the kernel is latency-bound per plan (dependent FP64 ops, divisions,
+ * shared-memory loads, shuffles and HBM round trips; tools/ub/lat.cu measures their latencies) and throughput comes from
  * running several hundred plans at once.  One pop is organised so that almost nothing sits on the serial chain:
  *
  *   warp 0  (search)  B1 when it was not prepared one pop ahead: one lane per control — exact FP64 end state,
@@ -46,13 +46,13 @@
 
 namespace mplb {
 
-/* tuning knobs (measured on the bench workload with tools/phase_timing.py, cycles per pop) */
+/* tuning knobs (chosen on the bench workload with tools/phase_timing.py, cycles per pop) */
 #ifndef MPLB_R
-#define MPLB_R 1 /* collision granules in flight per sampling thread: 1 -> 10.2k, 2 -> 10.9k, 4 -> 12.2k cycles per pop */
+#define MPLB_R 1 /* collision granules in flight per sampling thread: 2 and 4 cost more cycles per pop */
 #endif
 #ifndef MPLB_WIN
-#define MPLB_WIN 1 /* table slots fetched per probe (load factor <= 1/4): r01 at 3 CTAs/SM 2 -> 9.9k, 4 -> 10.9k cycles per pop; r02 at
-                      4-6 CTAs/SM one slot wins (+5 %): the second slot is bandwidth and registers for a 1-in-8 case */
+#define MPLB_WIN 1 /* table slots fetched per probe (load factor <= 1/4): at 4-6 CTAs/SM one slot wins; the second slot is
+                      bandwidth and registers for a 1-in-8 case */
 #endif
 #ifndef MPLB_LOAD_INV
 #define MPLB_LOAD_INV 4 /* table load factor bound 1/4 */
@@ -66,15 +66,15 @@ namespace mplb {
 #define MPLB_HCAP_SMALL 1024 /* shared-memory heap entries of the |U| > 32 instantiations when several plans share an SM */
 /* The ancestor ranges of the deep-heap pushes are fetched with the bulk asynchronous copy engine (cp.async.bulk + mbarrier,
  * UBLKCP / SYNCS in SASS): one copy per tree level, <= 23 per pop.  -DMPLB_NO_BULK_PREFETCH selects the 8-byte cp.async
- * (LDGSTS) variant; the two measure within 1.3 % of each other on the |U| = 125 workload (profiles/r02_tma_ab.md). */
+ * (LDGSTS) variant; the two measured within noise of each other on the |U| = 125 workload. */
 #if !defined(MPLB_NO_BULK_PREFETCH) && !defined(MPLB_BULK_PREFETCH)
 #define MPLB_BULK_PREFETCH 1
 #endif
 #ifndef MPLB_B1_INLINE
-#define MPLB_B1_INLINE __forceinline__ /* __noinline__ costs ~2k cycles per pop */
+#define MPLB_B1_INLINE __forceinline__ /* __noinline__ adds cycles to every pop */
 #endif
 #ifndef MPLB_SIFTUP_INLINE
-#define MPLB_SIFTUP_INLINE __forceinline__ /* __noinline__ costs ~1k cycles per pop */
+#define MPLB_SIFTUP_INLINE __forceinline__ /* __noinline__ adds cycles to every pop */
 #endif
 
 #define MPLB_INTERNAL_OVERFLOW 100 /* arena too small: host retries the plan in a larger tier */
@@ -1336,7 +1336,7 @@ astar_batch_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ Bat
             pf = H.hn()[0] & 0x7fffffff;
             const RowHdr *rh = reinterpret_cast<const RowHdr *>(rows + (size_t)pf * ROWB);
 #ifdef MPLB_BULK_ROW
-            /* A/B variant (profiles/r02_tma_ab.md): the whole state row (header + state, ROWB contiguous 16-byte aligned
+            /* A/B variant (slower, not the default): the whole state row (header + state, ROWB contiguous 16-byte aligned
              * bytes) arrives with ONE bulk asynchronous copy (TMA engine, cp.async.bulk) completing on an mbarrier, instead
              * of 3 + NS scalar loads. */
             {

@@ -2,7 +2,7 @@
 """Diagnostics: build libmplb with -DMPLB_PHASE_TIMING into a separate .so, run the bench batch once and print
 the clock64() cycle accumulators of thread 0 (search warp).  The TOTAL cycles per pop is reliable; the per-phase
 split is only indicative (clock64 is not ordered with barriers) — use the barrier-stall samples of an ncu capture for
-phase durations (see profiles/README.md).  Not part of the product."""
+phase durations.  Not part of the product."""
 import ctypes as C
 import os
 import subprocess

@@ -1,4 +1,4 @@
-// Latency calibration on B200 (diagnostics only): dependent-chain cycles per op for one warp.
+// Latency calibration (diagnostics only): dependent-chain cycles per op for one warp.
 #include <cstdio>
 #include <cuda_runtime.h>
 #define N 512
