@@ -90,6 +90,15 @@ typedef struct mplb_prim_trace {
   int32_t key[16];   /* lattice ints of tn (waypoint.h:92-125 order), key[15] = count */
 } mplb_prim_trace;
 
+/* One collision sample of env_map.h:99-104 as the search kernel's filtered sampler sees it (parity artefact). */
+typedef struct mplb_sample_probe {
+  int32_t state, control, k;   /* k-th sample time of the control's divisor */
+  int32_t sure;                /* filter decided without falling back */
+  int32_t cell_fast[3], cell_exact[3];
+  double t;
+  double w[3];                 /* filtered cell coordinate minus 0.5, as the filter computed it */
+} mplb_sample_probe;
+
 /* One search node (State<Coord>, state_space.h:36-70) of a retained single plan. */
 typedef struct mplb_node {
   double state[13];  /* stored coord = first discoverer's state (graph_search.h:84-88) */
@@ -313,6 +322,13 @@ int mplb_get_open(mplb_planner *p, int32_t *node_ids, int cap);        /* return
 
 /* env_map::get_succ (env_map.h:147-172) for n arbitrary states: rows [n * |U|]. HOST buffers. */
 int mplb_expand(mplb_planner *p, const mplb_waypoint *states, int n, mplb_prim_trace *rows);
+
+/* The search kernel's filtered collision sampler on n arbitrary states (plain map only, like mplb_expand): for every
+ * state and every control whose primitive needs sampling, one row per sample time, in no particular order.  Returns
+ * the number of rows (may exceed cap; only the first cap are written, rows may be NULL with cap = 0).  use_fast and
+ * fast_delta (either may be NULL) receive the configuration's filter switch and guard band in cells.  HOST buffers. */
+int mplb_probe_samples(mplb_planner *p, const mplb_waypoint *states, int n, mplb_sample_probe *rows, int cap,
+                       int32_t *use_fast, double *fast_delta);
 
 /* Correctly rounded sin/cos as the yaw branch evaluates them (primitive.h:520, env_map.h:125), computed on the device:
  * x, s, c are HOST arrays of n doubles, |x| < 2^20.  Parity artefact: tests compare it with the oracle and mpmath. */

@@ -18,6 +18,8 @@ RESULT_DTYPE = np.dtype([("status", "i4"), ("n_seg", "i4"), ("cost", "f8"), ("po
                          ("n_valid", "i8"), ("pop_hash", "u8"), ("closed_hash", "u8"), ("device_ms", "f8")], align=True)
 TRACE_DTYPE = np.dtype([("verdict", "i4"), ("n", "i4"), ("n_tested", "i4"), ("block_idx", "i4"), ("cost", "f8"),
                         ("succ", "f8", 13), ("key", "i4", 16)], align=True)
+PROBE_DTYPE = np.dtype([("state", "i4"), ("control", "i4"), ("k", "i4"), ("sure", "i4"), ("cell_fast", "i4", 3),
+                        ("cell_exact", "i4", 3), ("t", "f8"), ("w", "f8", 3)], align=True)
 NODE_DTYPE = np.dtype([("state", "f8", 13), ("g", "f8"), ("h", "f8"), ("key", "i4", 16), ("opened", "i4"),
                        ("closed", "i4"), ("parent", "i4"), ("action", "i4")], align=True)
 LPA_NODE_DTYPE = np.dtype([("key", "i4", 16), ("state", "f8", 13), ("g", "f8"), ("rhs", "f8"), ("h", "f8"), ("opened", "i4"),
@@ -58,6 +60,7 @@ SYMBOLS = {
     "mplb_get_pop_log": (_I, [_VP, _VP, _I]),
     "mplb_get_open": (_I, [_VP, _VP, _I]),
     "mplb_expand": (_I, [_VP, _VP, _I, _VP]),
+    "mplb_probe_samples": (_I, [_VP, _VP, _I, _VP, _I, _VP, _VP]),
     "mplb_last_batch_stats": (_I, [_VP, _VP, _VP, _VP]),
     "mplb_comm_unique_id": (_I, [_VP]),
     "mplb_comm_create": (_I, [_VP, _I, _I, _VP]),

@@ -516,8 +516,22 @@ int build_cfg(mplb_planner *p, int control) {
   c.ttab = p->d_ttab.p; c.toff = p->d_toff.p; c.tcnt = p->d_tcnt.p; c.n_hi = n_hi;
   c.tt_total = (int)ttab.size();
   c.inv_res = 1.0 / m->res;
-  /* filtered sampling (sample_blocked_filtered): FP64 Horner in cells; magnitude bound M = largest cell coordinate
-   * + sum of the largest displacement terms; evaluation error < 2^-45 * M, guard band 2^-40 * M. */
+  /* Guard band of the filtered sampler (filtered_w, clear_of_tie), in cells.  u = 2^-53 is the unit roundoff.
+   * M = largest cell coordinate a sampled parent can have (map extent + margin, maxc + margin_cells) + the largest
+   * displacement terms over one primitive (dsum: the dynamic bounds of a validated primitive, and |u| for the top
+   * coefficient, times dt^d / d! / res) + 2.  P = largest absolute coordinate a sample can take, in metres:
+   * max over the axes of |origin| + extent + margin.
+   * - The filter's w differs from the real value y = (p(t) - origin)/res - 0.5 by less than 8u * M: y0, the
+   *   coefficients and the Horner steps each round once or twice relative to numbers bounded by M.  Documented (and
+   *   tested) as < 2^-45 * M.
+   * - The reference's own value y_ref = fl(fl(fl(p) - origin)/res) - 0.5 (mu:103-108) differs from y by its rounding of
+   *   p (pr:128-131): the last add p = s + p0 happens at the magnitude of the absolute coordinate, <= u * P metres or
+   *   u * P / res cells, plus roundings relative to the cell coordinate and displacement, < 8u * M.
+   * (|p| <= P holds for every sample that can land inside the map: one farther out is outside whichever neighbouring
+   * cell it rounds to.)
+   * So |w - y_ref| < 2^-49 * M + 2^-53 * P / res, and the band 2^-40 * M + 2^-50 * P / res holds it with 8x headroom
+   * on the term that grows with the origin (UTM-style map frames: origins of 5e5 .. 1e7 m).  That term stays small
+   * enough for use_fast at such origins (about 2e-7 cells at 1e7 m and res = 0.05). */
   {
     double bnd[5] = {0, p->v_max, p->a_max, p->j_max, 0};
     bnd[ord] = umax; /* the control itself is the top coefficient */
@@ -528,9 +542,13 @@ int build_cfg(mplb_planner *p, int control) {
       if (!(bnd[d] > 0) && d < ord) known = false;
       dsum += std::fabs(bnd[d]) * tp / fact / m->res;
     }
-    double maxc = 0;
-    for (int i = 0; i < p->dim; i++) maxc = std::max(maxc, (double)m->nd[i]);
-    double delta = std::ldexp(maxc + margin_cells(vmax_eff, p->dt, m->res) + dsum + 2.0, -40);
+    double maxc = 0, maxp = 0;
+    const double margin_m = std::max(2.0, 2.0 * vmax_eff * p->dt);
+    for (int i = 0; i < p->dim; i++) {
+      maxc = std::max(maxc, (double)m->nd[i]);
+      maxp = std::max(maxp, std::fabs(m->origin[i]) + m->nd[i] * m->res + margin_m);
+    }
+    double delta = std::ldexp(maxc + margin_cells(vmax_eff, p->dt, m->res) + dsum + 2.0, -40) + std::ldexp(maxp / m->res, -50);
     c.use_fast = (known && n_hi < MPLB_NCAP && c.tt_total <= MPLB_TT_CAP && delta <= 1e-6) ? 1 : 0;
     c.fast_delta = delta;
   }
@@ -644,8 +662,12 @@ int build_cfg(mplb_planner *p, int control) {
       int f = ax * ord + d;
       long long lo, hi;
       if (d == 0) {
-        lo = (long long)std::floor((m->origin[ax] - margin) / 0.01) - 2;
-        hi = (long long)std::ceil((m->origin[ax] + m->nd[ax] * m->res + margin) / 0.01) + 2;
+        /* the reference's (int)std::round(pos / 0.01) (wp:97-99) is only defined while the quotient fits an int */
+        const double qlo = std::floor((m->origin[ax] - margin) / 0.01) - 2, qhi = std::ceil((m->origin[ax] + m->nd[ax] * m->res + margin) / 0.01) + 2;
+        if (!(qlo >= -2147483648.0 && qhi <= 2147483647.0))
+          return fail(MPLB_ERR_ARG, "map too far from the origin: lattice position keys round(pos / 0.01) leave the int32 range (|pos| must stay below about 2.1e7)");
+        lo = (long long)qlo;
+        hi = (long long)qhi;
       } else {
         double B = bounds[d] > 0 ? bounds[d] : 100.0;
         hi = (long long)std::ceil(B / 0.1) + 2;
@@ -1674,6 +1696,48 @@ int mplb_expand(mplb_planner *p, const mplb_waypoint *states, int n, mplb_prim_t
   cudaFree(d_r);
   if (e != cudaSuccess) return fail(MPLB_ERR_CUDA, std::string("expand: ") + cudaGetErrorString(e));
   return MPLB_OK;
+}
+
+int mplb_probe_samples(mplb_planner *p, const mplb_waypoint *states, int n, mplb_sample_probe *rows, int cap,
+                       int32_t *use_fast, double *fast_delta) {
+  if (!p || (n > 0 && !states) || (cap > 0 && !rows)) return fail(MPLB_ERR_ARG, "null argument");
+  if (n <= 0) return 0;
+  if (cap < 0) cap = 0;
+  if (set_device_of(p->device)) return fail(MPLB_ERR_CUDA, "cannot select the planner's device");
+  int rc = build_cfg(p, states[0].control);
+  if (rc != MPLB_OK) return rc;
+  const DevCfg &c = p->cfg;
+  if (c.pot || c.region || c.use_yaw) return fail(MPLB_ERR_STATE, "mplb_probe_samples probes the plain-map sampler only (no search region / potential map / yaw controls)");
+  if (use_fast) *use_fast = c.use_fast;
+  if (fast_delta) *fast_delta = c.fast_delta;
+  mplb_waypoint *d_s = nullptr;
+  mplb_sample_probe *d_r = nullptr;
+  int *d_count = nullptr;
+  CUDA_TRY(cudaMalloc((void **)&d_s, (size_t)n * sizeof(mplb_waypoint)));
+  CUDA_TRY(cudaMalloc((void **)&d_count, sizeof(int)));
+  if (cap > 0) CUDA_TRY(cudaMalloc((void **)&d_r, (size_t)cap * sizeof(mplb_sample_probe)));
+  CUDA_TRY(cudaMemcpy(d_s, states, (size_t)n * sizeof(mplb_waypoint), cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemset(d_count, 0, sizeof(int)));
+  int grid = std::min(n, 148 * 8);
+#define PROBE_CALL(D, O, M)                                                                                 \
+  do {                                                                                                      \
+    size_t smem = sizeof(PlanSmem<D, O, M>);                                                                \
+    auto kern = probe_samples_kernel<D, O, M>;                                                              \
+    if (smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
+    kern<<<grid, MPLB_NT, smem>>>(c, d_s, n, d_r, cap, d_count);                                            \
+  } while (0)
+  DISPATCH(c.dim, c.ord, c.nU, PROBE_CALL);
+#undef PROBE_CALL
+  g_launches++;
+  int count = 0;
+  cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) e = cudaMemcpy(&count, d_count, sizeof(int), cudaMemcpyDeviceToHost);
+  if (e == cudaSuccess && cap > 0) e = cudaMemcpy(rows, d_r, (size_t)std::min(count, cap) * sizeof(mplb_sample_probe), cudaMemcpyDeviceToHost);
+  cudaFree(d_s);
+  cudaFree(d_r);
+  cudaFree(d_count);
+  if (e != cudaSuccess) return fail(MPLB_ERR_CUDA, std::string("probe_samples: ") + cudaGetErrorString(e));
+  return count;
 }
 
 #ifdef MPLB_PHASE_TIMING

@@ -722,6 +722,23 @@ __device__ __forceinline__ void expand_b1(const DevCfg &c, const SM &S, EBT &E, 
   E.nid[i] = -1;
 }
 
+/* Filtered sampling (see filtered_w), per launch: the top polynomial coefficient u / ORD! of control i, in cells. */
+template <int DIM, int ORD, class SM>
+__device__ __forceinline__ void filter_top(const DevCfg &c, SM &S, int i) {
+  const double fact = (ORD == 1) ? 1.0 : (ORD == 2) ? 2.0 : (ORD == 3) ? 6.0 : 24.0;
+  for (int ax = 0; ax < 3; ax++) S.Au[i * 3 + ax] = (ax < DIM) ? c.U[i * 3 + ax] / fact * c.inv_res : 0.0;
+}
+
+/* Filtered sampling, per pop: the sampling base of the node in E.st on axis ax (parent cell coordinate and lower
+ * polynomial coefficients, in cells). */
+template <int DIM, int ORD, class EBT>
+__device__ __forceinline__ void filter_base(const DevCfg &c, EBT &E, int ax) {
+  E.y0[ax] = dmul(dsub(E.st[ax], c.origin[ax]), c.inv_res);
+  if (ORD >= 2) E.Ap[0 * 3 + ax] = dmul(E.st[DIM + ax], c.inv_res);
+  if (ORD >= 3) E.Ap[1 * 3 + ax] = dmul(dmul(E.st[2 * DIM + ax], 0.5), c.inv_res);
+  if (ORD >= 4) E.Ap[2 * 3 + ax] = dmul(div_exact(E.st[3 * DIM + ax], 6.0), c.inv_res);
+}
+
 /* B1 for all controls of one node by ONE warp, plus the flat sample list (granules) and the sampling base.
  * E.st / E.pk0 / E.pk1 must hold the node's state and packed lattice key. */
 template <int DIM, int ORD, int NB, class SM, class EBT>
@@ -729,13 +746,7 @@ __device__ MPLB_B1_INLINE void b1_warp(const DevCfg &c, const SM &S, EBT &E, int
   if (lane == 0) E.key_bad = 0;
   if (EBT::NS > DIM * ORD && lane == 31 && c.use_yaw && c.yaw_max > 0.0)
     trig::sincos_cr(normalize_angle(E.st[DIM * ORD]), &E.sy0, &E.cy0); /* evaluate(0) normalises the yaw too (pr:328) */
-  if (fast && lane < DIM) { /* sampling base (cells): parent cell coordinate and lower polynomial coefficients */
-    const int ax = lane;
-    E.y0[ax] = dmul(dsub(E.st[ax], c.origin[ax]), c.inv_res);
-    if (ORD >= 2) E.Ap[0 * 3 + ax] = dmul(E.st[DIM + ax], c.inv_res);
-    if (ORD >= 3) E.Ap[1 * 3 + ax] = dmul(dmul(E.st[2 * DIM + ax], 0.5), c.inv_res);
-    if (ORD >= 4) E.Ap[2 * 3 + ax] = dmul(div_exact(E.st[3 * DIM + ax], 6.0), c.inv_res);
-  }
+  if (fast && lane < DIM) filter_base<DIM, ORD>(c, E, lane);
   __syncwarp();
   int gbase = 0;
 #pragma unroll
@@ -780,24 +791,36 @@ __device__ __noinline__ bool sample_blocked_exact(const DevCfg &c, const SM &S, 
   return brick_occupied<DIM>(c, pn[0], pn[1], pn[2]);
 }
 
-/* Filtered sample.  The cell coordinate y = (p(t) - origin)/res is evaluated as one FP64 Horner chain in cells
- * (parent coordinate y0 and lower coefficients per pop, top coefficient per control; FMA allowed because the
- * value is only used to decide a rounding).  Its error is < 2^-45 * (|y| + displacement terms); when y - 0.5 is
- * farther than c.fast_delta (>= 2^-40 * the same magnitude, set by the host) from a rounding tie, round(y - 0.5)
- * equals the reference's round((p - origin)/res - 0.5) (mu:103-108).  Otherwise *sure is cleared and the caller
- * evaluates the exact formula. */
+/* Filtered cell coordinate of one axis.  The cell coordinate minus one half, w = (p(t) - origin)/res - 0.5, is evaluated
+ * as one FP64 Horner chain in cells (parent coordinate y0 and lower coefficients per pop, filter_base; top coefficient
+ * per control, filter_top; FMA allowed because the value is only used to decide a rounding).  Its distance from the real
+ * value is < 2^-45 * M, M = the host's magnitude bound (build_cfg).  When w is farther than c.fast_delta from a rounding
+ * tie (clear_of_tie), round(w) equals the reference's round((p - origin)/res - 0.5) (mu:103-108): c.fast_delta also
+ * covers the reference's own rounding of that expression, see build_cfg.  Otherwise the caller evaluates the exact
+ * formula. */
+template <int ORD, class SM, class EBT>
+__device__ __forceinline__ double filtered_w(const SM &S, const EBT &E, int i, int ax, double t) {
+  double dy = S.Au[i * 3 + ax];
+#pragma unroll
+  for (int d = ORD - 2; d >= 0; d--) dy = __fma_rn(dy, t, E.Ap[d * 3 + ax]);
+  return __dsub_rn(__fma_rn(dy, t, E.y0[ax]), 0.5);
+}
+/* wm = magic_add(w): true when round(w) = magic_int(wm) is decided by the filter */
+__device__ __forceinline__ bool clear_of_tie(const DevCfg &c, double w, double wm) {
+  return fabs(__dsub_rn(w, magic_rint(wm))) < 0.5 - c.fast_delta;
+}
+
+/* Filtered sample: the filtered cell on every axis, then the occupancy bit.  *sure is cleared when an axis is too close
+ * to a tie (the return value is then meaningless and the caller evaluates sample_blocked_exact). */
 template <int DIM, int ORD, class SM, class EBT>
 __device__ __forceinline__ bool sample_blocked_filtered(const DevCfg &c, const SM &S, const EBT &E, int i, double t, bool *sure) {
   int pn[3] = {0, 0, 0};
   bool ok = true, outside = false;
 #pragma unroll
   for (int ax = 0; ax < DIM; ax++) {
-    double dy = S.Au[i * 3 + ax];
-#pragma unroll
-    for (int d = ORD - 2; d >= 0; d--) dy = __fma_rn(dy, t, E.Ap[d * 3 + ax]);
-    double w = __dsub_rn(__fma_rn(dy, t, E.y0[ax]), 0.5);
+    double w = filtered_w<ORD>(S, E, i, ax, t);
     double wm = magic_add(w);
-    ok = ok && (fabs(__dsub_rn(w, magic_rint(wm))) < 0.5 - c.fast_delta);
+    ok = ok && clear_of_tie(c, w, wm);
     pn[ax] = magic_int(wm);
     outside = outside || pn[ax] < 0 || pn[ax] >= c.nd[ax];
   }
@@ -1049,12 +1072,9 @@ __device__ __forceinline__ bool cell_filtered(const DevCfg &c, const SM &S, cons
   bool ok = true, outside = false;
 #pragma unroll
   for (int ax = 0; ax < DIM; ax++) {
-    double dy = S.Au[i * 3 + ax];
-#pragma unroll
-    for (int d = ORD - 2; d >= 0; d--) dy = __fma_rn(dy, t, E.Ap[d * 3 + ax]);
-    double w = __dsub_rn(__fma_rn(dy, t, E.y0[ax]), 0.5);
+    double w = filtered_w<ORD>(S, E, i, ax, t);
     double wm = magic_add(w);
-    ok = ok && (fabs(__dsub_rn(w, magic_rint(wm))) < 0.5 - c.fast_delta);
+    ok = ok && clear_of_tie(c, w, wm);
     pn[ax] = magic_int(wm);
     outside = outside || pn[ax] < 0 || pn[ax] >= c.nd[ax];
   }
@@ -1166,8 +1186,7 @@ astar_batch_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ Bat
     double J = 0.0;
     for (int ax = 0; ax < DIM; ax++) { double u = c.U[i * 3 + ax]; J = dadd(J, dmul(dmul(u, u), c.dt)); } /* pr:92-122,403-407 */
     S.cost[i] = dadd(J, dmul(c.w, c.dt));                                                                /* eb:343-345 */
-    const double fact = (ORD == 1) ? 1.0 : (ORD == 2) ? 2.0 : (ORD == 3) ? 6.0 : 24.0;
-    for (int ax = 0; ax < 3; ax++) S.Au[i * 3 + ax] = (ax < DIM) ? c.U[i * 3 + ax] / fact * c.inv_res : 0.0;
+    filter_top<DIM, ORD>(c, S, i);
   }
   if (fast) {
     for (int i = tid; i < MPLB_NCAP; i += MPLB_NT) { S.toff_s[i] = (i <= c.n_hi) ? c.toff[i] : 0; S.tcnt_s[i] = (i <= c.n_hi) ? c.tcnt[i] : 0; }
@@ -1812,6 +1831,67 @@ __global__ void __launch_bounds__(MPLB_NT) expand_trace_kernel(const __grid_cons
       for (int f = 0; f < NS; f++) r.key[f] = ints[f];
       r.key[15] = NS;
       rows[(size_t)s * c.nU + i] = r;
+    }
+  }
+}
+
+/* ---------------------------------------------------------------- the filtered sampler on arbitrary states (parity artefact)
+ * B1 as the search runs it, then, for every control whose primitive needs sampling (verdict 5), every sample time of its
+ * divisor: the filtered cell (filtered_w, clear_of_tie, with the search's per-launch and per-pop set-up) next to the exact one
+ * (cell_exact).  Rows are appended in no particular order through *count; only the first `cap` are stored. */
+template <int DIM, int ORD, int NB>
+__global__ void __launch_bounds__(MPLB_NT) probe_samples_kernel(const __grid_constant__ DevCfg c, const mplb_waypoint *states,
+                                                                int n_states, mplb_sample_probe *rows, int cap, int *count) {
+  constexpr int NW = MPLB_NT / 32;
+  using SM = PlanSmem<DIM, ORD, NB>;
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  SM &S = *reinterpret_cast<SM *>(smem_raw);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  for (int i = tid; i < c.nU * 3; i += MPLB_NT) { S.U[i] = c.U[i]; S.Ut[i] = Axis<ORD>::top_of(c.U[i]); }
+  for (int i = tid; i < c.nU; i += MPLB_NT) filter_top<DIM, ORD>(c, S, i);
+  if (c.use_fast) for (int i = tid; i < MPLB_NCAP; i += MPLB_NT) S.tcnt_s[i] = (i <= c.n_hi) ? c.tcnt[i] : 0;
+  typename SM::EB &E = S.eb[0];
+  for (int s = blockIdx.x; s < n_states; s += gridDim.x) {
+    __syncthreads();
+    if (tid == 0) {
+      const mplb_waypoint &st = states[s];
+      for (int ax = 0; ax < DIM; ax++) {
+        E.st[ax] = st.pos[ax];
+        if (ORD >= 2) E.st[DIM + ax] = st.vel[ax];
+        if (ORD >= 3) E.st[2 * DIM + ax] = st.acc[ax];
+        if (ORD >= 4) E.st[3 * DIM + ax] = st.jrk[ax];
+      }
+      int ints0[DIM * ORD];
+      lattice_ints<DIM, ORD>(E.st, ints0);
+      if (!pack_key_nohash<DIM, ORD>(c, ints0, E.pk0, E.pk1)) { E.pk0 = ~0ull; E.pk1 = ~0ull; }
+    }
+    __syncthreads();
+    for (int i = tid; i < c.nU; i += MPLB_NT) expand_b1<DIM, ORD>(c, S, E, i);
+    if (tid < DIM) filter_base<DIM, ORD>(c, E, tid);
+    __syncthreads();
+    for (int i = warp; i < c.nU; i += NW) {
+      if (E.verdict[i] != 5) continue;
+      const double *tt = c.ttab + c.toff[E.nsamp[i]];
+      for (int k = lane; k < E.cnt[i]; k += 32) {
+        mplb_sample_probe r;
+        r.state = s; r.control = i; r.k = k;
+        r.t = tt[k];
+        bool sure = true;
+        int pe[3] = {0, 0, 0};
+        cell_exact<DIM, ORD>(c, S, E.st, i, r.t, pe);
+        for (int ax = 0; ax < 3; ax++) {
+          r.w[ax] = 0.0; r.cell_fast[ax] = 0; r.cell_exact[ax] = pe[ax];
+          if (ax < DIM) {
+            const double w = filtered_w<ORD>(S, E, i, ax, r.t), wm = magic_add(w);
+            sure = sure && clear_of_tie(c, w, wm);
+            r.w[ax] = w;
+            r.cell_fast[ax] = magic_int(wm);
+          }
+        }
+        r.sure = sure ? 1 : 0;
+        const int slot = atomicAdd(count, 1);
+        if (slot < cap) rows[slot] = r;
+      }
     }
   }
 }

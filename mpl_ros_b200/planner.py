@@ -613,6 +613,19 @@ class MapPlanner:
         check(lib().mplb_expand(self._h, ptr(states), n, ptr(rows)))
         return rows
 
+    def probe_samples(self, states):
+        """The search kernel's filtered collision sampler on arbitrary states: one row per (state, control needing
+        sampling, sample time), sorted by (state, control, k).  Returns (rows, use_fast, fast_delta)."""
+        n = len(states)
+        uf, fd = C.c_int32(), C.c_double()
+        cnt = check(lib().mplb_probe_samples(self._h, ptr(states), n, None, 0, C.byref(uf), C.byref(fd)))
+        rows = np.zeros(max(cnt, 1), dtype=_lib.PROBE_DTYPE)
+        got = check(lib().mplb_probe_samples(self._h, ptr(states), n, ptr(rows), rows.size, None, None))
+        assert got == cnt, (got, cnt)
+        rows = rows[:cnt]
+        rows = rows[np.lexsort((rows["k"], rows["control"], rows["state"]))]
+        return rows, int(uf.value), float(fd.value)
+
 
 class OccMapPlanner(MapPlanner):  # map_planner.h:122
     def __init__(self, verbose=False):

@@ -25,6 +25,7 @@ def test_struct_layouts_match_header():
     import oracle
     assert _lib.WAYPOINT_DTYPE.itemsize == 120 and _lib.RESULT_DTYPE.itemsize == 80
     assert _lib.TRACE_DTYPE.itemsize == 4 * 4 + 8 + 13 * 8 + 16 * 4
+    assert _lib.PROBE_DTYPE.itemsize == 4 * 4 + 6 * 4 + 8 + 3 * 8
     # the oracle mirrors the same layouts so tests can share buffers
     assert oracle.WAYPOINT_DTYPE == _lib.WAYPOINT_DTYPE and oracle.RESULT_DTYPE == _lib.RESULT_DTYPE
 
