@@ -8,7 +8,7 @@ import subprocess
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 INC = os.path.join(HERE, "..", "include", "mplb.h")
-SRC = os.path.join(CSRC, "mplb.cu")  # the search runtime (tools/phase_timing.py builds this unit alone)
+SRC = os.path.join(CSRC, "mplb.cu")  # the search runtime
 _COMMON = [INC, os.path.join(CSRC, "mplb_internal.h")]
 UNITS = {
     "mplb.cu": [os.path.join(CSRC, h) for h in ("mplb_search.cuh", "mplb_device.cuh", "mplb_trig.cuh")] + _COMMON,

@@ -47,9 +47,6 @@
 namespace mplb {
 
 /* tuning knobs (chosen on the bench workload with tools/phase_timing.py, cycles per pop) */
-#ifndef MPLB_R
-#define MPLB_R 1 /* collision granules in flight per sampling thread: 2 and 4 cost more cycles per pop */
-#endif
 #ifndef MPLB_WIN
 #define MPLB_WIN 1 /* table slots fetched per probe (load factor <= 1/4): at 4-6 CTAs/SM one slot wins; the second slot is
                       bandwidth and registers for a 1-in-8 case */
@@ -196,7 +193,7 @@ struct ExpBuf {
   int cnt[MAXU];     /* samples to test */
   int first[MAXU];   /* first blocked sample index or INT_MAX */
   int nid[MAXU];     /* node id of the successor after relaxation (for state forwarding) */
-  int gbase[MAXU];   /* first granule of the control in gl[] (cost-shaping kernels sum its sample terms in order) */
+  int gbase[MAXU];   /* first granule of the control in gl[] (cost-shaping kernels only: they sum its sample terms in order) */
   double dts[MAXU];  /* sample spacing T/n (em:98), cost-shaping kernels only */
   double cy0, sy0;   /* cos/sin of the node's yaw (yaw controls) */
   unsigned int gl[GCAP];     /* granule: control | first sample k0 << 8 | sample count << 16 ... */
@@ -209,6 +206,9 @@ struct PlanSmem {
   static constexpr int NS = NP + (POT ? 1 : 0);
   static constexpr int MAXU = 32 * NB;
   static constexpr int NBUF = 2; /* expansion records: B1 of the next pop is pipelined into the second one */
+  /* granule order of the sample list (b1_warp): wave-major in the plain kernels, so that the sampler can skip the granules
+   * behind a control's first blocked sample; control-major in the cost-shaping kernels, which need every sample's term */
+  static constexpr bool WAVE_MAJOR = !POT;
   typedef ExpBuf<DIM, ORD, MAXU, POT ? 1 : 0> EB;
   EB eb[NBUF];
   int cur_buf;
@@ -740,7 +740,11 @@ __device__ __forceinline__ void filter_base(const DevCfg &c, EBT &E, int ax) {
 }
 
 /* B1 for all controls of one node by ONE warp, plus the flat sample list (granules) and the sampling base.
- * E.st / E.pk0 / E.pk1 must hold the node's state and packed lattice key. */
+ * E.st / E.pk0 / E.pk1 must hold the node's state and packed lattice key.
+ * Granule q of a control holds its samples 8q .. 8q + 7.  SM::WAVE_MAJOR: the list holds granule 0 of every sampled
+ * control, then granule 1 of every control that has one, and so on, so that the sampler reaches a control's later
+ * granules after its earlier ones have had the chance to find a blocked sample.  Otherwise: all granules of control 0,
+ * then all of control 1, ... (E.gbase[i] is the first granule of control i). */
 template <int DIM, int ORD, int NB, class SM, class EBT>
 __device__ MPLB_B1_INLINE void b1_warp(const DevCfg &c, const SM &S, EBT &E, int lane, bool fast) {
   if (lane == 0) E.key_bad = 0;
@@ -749,24 +753,46 @@ __device__ MPLB_B1_INLINE void b1_warp(const DevCfg &c, const SM &S, EBT &E, int
   if (fast && lane < DIM) filter_base<DIM, ORD>(c, E, lane);
   __syncwarp();
   int gbase = 0;
+  int ng[NB];
 #pragma unroll
   for (int b = 0; b < NB; b++) {
     const int i = b * 32 + lane;
-    int ng = 0;
+    ng[b] = 0;
     if (i < c.nU) {
       expand_b1<DIM, ORD>(c, S, E, i);
-      if (fast && E.verdict[i] == 5) ng = (E.cnt[i] + 7) >> 3;
+      if (fast && E.verdict[i] == 5) ng[b] = (E.cnt[i] + 7) >> 3;
     }
-    int incl = ng; /* warp scan of the granule counts */
+    if (SM::WAVE_MAJOR) continue;
+    int incl = ng[b]; /* warp scan of the granule counts */
 #pragma unroll
     for (int d = 1; d < 32; d <<= 1) { int v = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= d) incl += v; }
-    int excl = gbase + incl - ng;
+    int excl = gbase + incl - ng[b];
     if (i < c.nU) { E.gbase[i] = excl; if ((c.pot || c.use_yaw) && E.nsamp[i] > 0) E.dts[i] = ddiv(c.dt, (double)E.nsamp[i]); }
-    for (int q = 0; q < ng; q++) {
+    for (int q = 0; q < ng[b]; q++) {
       E.gl[excl + q] = (unsigned)i | ((unsigned)(q * 8) << 8) | ((unsigned)E.cnt[i] << 16);
       E.gl_t[excl + q] = (unsigned short)(S.toff_s[E.nsamp[i]] + q * 8);
     }
     gbase += __shfl_sync(0xffffffffu, incl, 31);
+  }
+  if (SM::WAVE_MAJOR) {
+    int ngmax = 0;
+#pragma unroll
+    for (int b = 0; b < NB; b++) ngmax = max(ngmax, ng[b]);
+    ngmax = __reduce_max_sync(0xffffffffu, ngmax);
+    const unsigned lt = (1u << lane) - 1u;
+    for (int q = 0; q < ngmax; q++) {
+#pragma unroll
+      for (int b = 0; b < NB; b++) {
+        const int i = b * 32 + lane;
+        const unsigned m = __ballot_sync(0xffffffffu, ng[b] > q);
+        if (ng[b] > q) {
+          const int g = gbase + __popc(m & lt);
+          E.gl[g] = (unsigned)i | ((unsigned)(q * 8) << 8) | ((unsigned)E.cnt[i] << 16);
+          E.gl_t[g] = (unsigned short)(S.toff_s[E.nsamp[i]] + q * 8);
+        }
+        gbase += __popc(m);
+      }
+    }
   }
   if (lane == 0) E.n_gran = gbase;
   __syncwarp();
@@ -1020,37 +1046,31 @@ __device__ __noinline__ void relax_serial(const DevCfg &c, SM &S, typename SM::E
   }
 }
 
-/* B2, flat form: thread `t` of `nthreads` sampling threads takes sample (t & 7) of granule (t >> 3) + k*(nthreads/8);
- * R granules are processed per pass with their loads issued together (independent dependency chains). */
+/* B2, flat form, plain kernels: thread `t` of `nthreads` sampling threads takes sample (t & 7) of granule
+ * (t >> 3) + j * (nthreads / 8) of the wave-major list.  (Handing the granules to octets through a shared counter instead
+ * measured no faster than not skipping at all.)
+ * A sample whose index k is >= E.first[u] at the time the thread reaches it is skipped and issues no brick load.  This is
+ * exact: E.first[u] only ever holds the index of a sample that was evaluated and found blocked, so a skipped sample has a
+ * larger index than some blocked sample and cannot be the first one.  Every value E.first[u] takes is >= the first blocked
+ * index k*, so k* is skipped only once E.first[u] == k*, i.e. once it is recorded.  The final atomicMin value is the true
+ * first blocked index, and first == INT_MAX still means that no sample is blocked (nothing is skipped then). */
 template <int DIM, int ORD, class SM, class EBT>
 __device__ __forceinline__ void sample_granules(const DevCfg &c, const SM &S, EBT &E, int t, int nthreads) {
-  const int gstep = nthreads >> 3;
   const int sub = t & 7;
-  constexpr int R = MPLB_R; /* granules in flight per thread */
-  for (int g0 = t >> 3; g0 < E.n_gran; g0 += R * gstep) {
-    unsigned info[R];
-    double st[R];
-    bool act[R], blk[R], sure[R];
-#pragma unroll
-    for (int r = 0; r < R; r++) {
-      const int g = g0 + gstep * r;
-      const bool in = g < E.n_gran;
-      info[r] = in ? E.gl[g] : 0u;
-      const int k = (int)((info[r] >> 8) & 0xffu) + sub;
-      act[r] = in && k < (int)(info[r] >> 16);
-      st[r] = act[r] ? S.tts[(int)E.gl_t[in ? g : 0] + sub] : 0.0;
-    }
-#pragma unroll
-    for (int r = 0; r < R; r++) {
-      sure[r] = true;
-      blk[r] = act[r] && sample_blocked_filtered<DIM, ORD>(c, S, E, (int)(info[r] & 0xffu), st[r], &sure[r]);
-    }
-#pragma unroll
-    for (int r = 0; r < R; r++) {
-      const int u = (int)(info[r] & 0xffu);
-      if (act[r] && !sure[r]) blk[r] = sample_blocked_exact<DIM, ORD>(c, S, E.st, u, st[r], nullptr);
-      if (blk[r]) atomicMin(&E.first[u], (int)((info[r] >> 8) & 0xffu) + sub);
-    }
+  const volatile int *first = E.first; /* lowered by the other octets while this one works */
+  for (int g = t >> 3; g < E.n_gran; g += nthreads >> 3) {
+    const unsigned info = E.gl[g];
+    const int u = (int)(info & 0xffu);
+    const int k = (int)((info >> 8) & 0xffu) + sub;
+    if (k >= (int)(info >> 16) || k >= first[u]) continue;
+#ifdef MPLB_PHASE_TIMING
+    if (sub == 0) atomicAdd(const_cast<unsigned long long *>(&S.dbg[2]), 1ull); /* granules evaluated */
+#endif
+    const double ts = S.tts[(int)E.gl_t[g] + sub];
+    bool sure = true;
+    bool blk = sample_blocked_filtered<DIM, ORD>(c, S, E, u, ts, &sure);
+    if (!sure) blk = sample_blocked_exact<DIM, ORD>(c, S, E.st, u, ts, nullptr);
+    if (blk) atomicMin(&E.first[u], k);
   }
 }
 

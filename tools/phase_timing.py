@@ -16,7 +16,7 @@ from mpl_ros_b200 import build as B  # noqa: E402
 
 out = os.path.join(ROOT, "mpl_ros_b200", os.environ.get("MPLB_PROF_SO", "libmplb_prof.so"))
 if "--build-only" in sys.argv or not os.path.exists(out):
-    subprocess.check_call([os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")] + B.NVCC_FLAGS + ["-DMPLB_PHASE_TIMING=" + os.environ.get("MPLB_PT", "1")] + os.environ.get("MPLB_DEFS", "").split() + ["-o", out, B.SRC])
+    subprocess.check_call([os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")] + B.NVCC_FLAGS + ["-DMPLB_PHASE_TIMING=" + os.environ.get("MPLB_PT", "1")] + os.environ.get("MPLB_DEFS", "").split() + ["-o", out] + [os.path.join(B.CSRC, u) for u in B.UNITS])
     if "--build-only" in sys.argv:
         sys.exit(0)
 from mpl_ros_b200 import _lib  # noqa: E402
@@ -54,7 +54,7 @@ assert L.mplb_debug_phase_cycles(pl._h, ph16.ctypes.data_as(C.c_void_p), len(s))
 ph = ph16[:, :8]
 dbg = ph16[:, 8:]
 print('dbg per pop', (dbg.sum(axis=0) / res['pops'].sum()).astype(int).tolist())
-print('counters per pop: fast_on %.3f samples %.1f granules %.1f hazards %.4f exact_samples %.3f' % tuple(dbg[:, k].sum() / res['pops'].sum() for k in (0, 1, 2, 3, 4)))
+print('per pop: decide cycles %.0f  store cycles %.0f  granules evaluated %.1f  hazards %.4f  exact samples %.3f' % tuple(dbg[:, k].sum() / res['pops'].sum() for k in (0, 1, 2, 3, 4)))
 names = ["P1 (miss path only) + bar1", "P2 probe issue + h + resolve", "P2 (unused)", "P2 wait at bar 2", "P3 relax: decide+stores",
          "P3 relax: heap ops", "P3 terminate+pop", "loop top (barrier C + checks)"]
 pops = res["pops"].astype(np.float64)
