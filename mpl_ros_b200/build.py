@@ -11,16 +11,18 @@ INC = os.path.join(HERE, "..", "include", "mplb.h")
 SRC = os.path.join(CSRC, "mplb.cu")  # the search runtime
 _COMMON = [INC, os.path.join(CSRC, "mplb_internal.h")]
 UNITS = {
-    "mplb.cu": [os.path.join(CSRC, h) for h in ("mplb_search.cuh", "mplb_device.cuh", "mplb_trig.cuh")] + _COMMON,
-    "mplb_trajsolve.cu": list(_COMMON),
-    "mplb_lpa.cu": [os.path.join(CSRC, h) for h in ("mplb_device.cuh", "mplb_lpa_core.h")] + _COMMON,
+    "mplb.cu": [os.path.join(CSRC, h) for h in ("mplb_search.cuh", "mplb_device.cuh", "mplb_trig.cuh", "mplb_ref.h")] + _COMMON,
+    "mplb_trajsolve.cu": [os.path.join(CSRC, "mplb_ref.h")] + _COMMON,
+    "mplb_lpa.cu": [os.path.join(CSRC, h) for h in ("mplb_lpa_core.h", "mplb_ref.h")] + _COMMON,
 }
 DEPS = [SRC] + UNITS["mplb.cu"]
 OUT = os.path.join(HERE, "libmplb.so")
 
 # -fmad=false: the reference is built without FMA contraction (MPL/CMakeLists.txt:5-8); the kernels also use
-# explicit __d*_rn intrinsics, the flag covers whatever remains.
-ARCH_FLAGS = ["-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-fmad=false"]
+# explicit __d*_rn intrinsics, the flag covers whatever remains.  -ffp-contract=off does the same for the host half of
+# mplb_ref.h's functions (prior-trajectory table, search-region builder), as in the host build of the LPA* core.
+ARCH_FLAGS = ["-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-fmad=false",
+              "-Xcompiler", "-ffp-contract=off"]
 NVCC_FLAGS = ["-shared", "-Xcompiler", "-fPIC"] + ARCH_FLAGS
 
 

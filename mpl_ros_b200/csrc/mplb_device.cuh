@@ -15,6 +15,7 @@
 #include <stdint.h>
 
 #include "../../include/mplb.h"
+#include "mplb_ref.h"
 
 namespace mplb {
 
@@ -30,10 +31,19 @@ namespace mplb {
                            batch is tail bound and prefers 256x3). */
 #endif
 
-__device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a, b); }
-__device__ __forceinline__ double dsub(double a, double b) { return __dsub_rn(a, b); }
-__device__ __forceinline__ double dmul(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ double ddiv(double a, double b) { return __ddiv_rn(a, b); }
+/* exact reference arithmetic shared with the rest of the library (mplb_ref.h) */
+using mplb_ref::dadd;
+using mplb_ref::dsub;
+using mplb_ref::dmul;
+using mplb_ref::ddiv;
+using mplb_ref::round_int;
+using mplb_ref::float_to_cell;
+using mplb_ref::normalize_angle;
+using mplb_ref::ray_setup;
+using mplb_ref::ray_point;
+using mplb_ref::khash_init;
+using mplb_ref::khash_step;
+using mplb_ref::khash_final;
 
 /* Rounding without the XU pipe.  Every FP64 conversion / rounding instruction (F2I, I2F, FRND, MUFU.RCP64H)
  * issues to the low-rate XU pipe and has a long latency on the serial chain of a pop; adding and subtracting
@@ -43,14 +53,6 @@ __device__ __forceinline__ double ddiv(double a, double b) { return __ddiv_rn(a,
 __device__ __forceinline__ double magic_add(double x) { return __dadd_rn(x, MPLB_MAGIC); }
 __device__ __forceinline__ double magic_rint(double xm) { return __dsub_rn(xm, MPLB_MAGIC); }
 __device__ __forceinline__ int magic_int(double xm) { return __double2loint(xm); }
-
-/* std::round (half away from zero), exact: x - trunc(x) is exactly representable. */
-__device__ __forceinline__ double round_haz(double x) {
-  double r = trunc(x);
-  if (fabs(dsub(x, r)) >= 0.5) r = dadd(r, copysign(1.0, x));
-  return r;
-}
-__device__ __forceinline__ int round_int(double x) { return __double2int_rz(round_haz(x)); }
 
 /* Device view of planner + map configuration (kernel parameter, by value). */
 struct DevCfg {
@@ -99,7 +101,8 @@ struct DevCfg {
 };
 
 /* ------------------------------------------------------------------------------------------------
- * Polynomial primitive on one axis (pr:21-198).  Coefficients c1..c5 (c0 is 0 for every control
+ * Polynomial primitive on one axis (pr:21-198), specialised per control order: the literal six-coefficient form is
+ * mplb_ref.h's Prim1; this one drops its structurally-zero terms.  Coefficients c1..c5 (c0 is 0 for every control
  * constructor pr:35-52).  For control order ORD the leading non-zero coefficient is c[5-ORD] = u.
  *   ORD 1 (VEL): c4 = u, c5 = p          ORD 2 (ACC): c3 = u, c4 = v, c5 = p
  *   ORD 3 (JRK): c2 = u, c3 = a, ...     ORD 4 (SNP): c1 = u, c2 = j, ...
@@ -199,11 +202,6 @@ struct Axis {
   }
 };
 
-/* mu:103-108  pn = round((pt - origin)/res - 0.5) */
-__device__ __forceinline__ int float_to_cell(double pt, double origin, double res) {
-  return round_int(dsub(ddiv(dsub(pt, origin), res), 0.5));
-}
-
 /* Occupancy test of an inside cell through the bit-bricks (value == 100, mu:48). */
 template <int DIM>
 __device__ __forceinline__ bool brick_occupied(const DevCfg &c, int x, int y, int z) {
@@ -216,21 +214,6 @@ __device__ __forceinline__ bool brick_occupied(const DevCfg &c, int x, int y, in
     unsigned bit = (x & 7) | ((y & 7) << 3);
     return (__ldg(&c.bricks[b]) >> bit) & 1ull;
   }
-}
-
-/* 64-bit mixing hash of the lattice ints — same definition as the oracle's key_hash(). */
-__device__ __forceinline__ unsigned long long khash_init() { return 0x243F6A8885A308D3ull; }
-__device__ __forceinline__ unsigned long long khash_step(unsigned long long h, int v) {
-  h ^= (unsigned long long)(unsigned int)v;
-  h *= 0x9E3779B97F4A7C15ull;
-  h ^= h >> 32;
-  return h;
-}
-__device__ __forceinline__ unsigned long long khash_final(unsigned long long h) {
-  h ^= h >> 30; h *= 0xBF58476D1CE4E5B9ull;
-  h ^= h >> 27; h *= 0x94D049BB133111EBull;
-  h ^= h >> 31;
-  return h;
 }
 
 /* Lattice ints of a state (wp:92-125): pos/0.01, derivatives/0.1, axis-major order. st[d*DIM + axis]. */

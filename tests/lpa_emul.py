@@ -9,7 +9,8 @@ from oracle.lpa import LpaMixin, map_set_cells
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "cpp", "lpa_emul.cpp")
-CORE = os.path.join(HERE, "..", "mpl_ros_b200", "csrc", "mplb_lpa_core.h")
+CSRC = os.path.join(HERE, "..", "mpl_ros_b200", "csrc")
+DEPS = [SRC, os.path.join(CSRC, "mplb_lpa_core.h"), os.path.join(CSRC, "mplb_ref.h")]
 _LIBS = {}
 
 
@@ -17,7 +18,7 @@ def lib(reverse=False):
     """reverse: the build whose lane loops run 31 .. 0 inside every phase (the result must not depend on that order)"""
     if reverse not in _LIBS:
         SO = os.path.join(HERE, "cpp", "_lpa_emul_rev.so" if reverse else "_lpa_emul.so")
-        if not os.path.exists(SO) or os.path.getmtime(SO) < max(os.path.getmtime(SRC), os.path.getmtime(CORE)):
+        if not os.path.exists(SO) or os.path.getmtime(SO) < max(os.path.getmtime(d) for d in DEPS):
             subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared", "-Wall"] +
                                   (["-DLPA_REVERSE_LANES"] if reverse else []) + ["-o", SO + ".tmp", SRC])
             os.replace(SO + ".tmp", SO)
