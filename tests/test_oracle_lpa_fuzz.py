@@ -21,13 +21,19 @@ from test_oracle_fuzz_vs_reference import rand_case
 HAVE_REF = ref.available()
 
 
-def run_sequence(seed, dim, impls, rounds=4):
+def sequence_case(seed, dim):
+    """(rng, (nd, origin, res, data, ctl, U, prm, start, goal, vel)) of sequence `seed`; the rng continues into the steps."""
     rng = np.random.default_rng(7000 + seed)
     nd, origin, res, data, ctl, U, prm, start, goal, vel = rand_case(rng, dim)
     prm = {k: v for k, v in prm.items() if k in ("v_max", "a_max", "j_max", "dt", "w", "epsilon", "tol_pos", "max_num")}
     if prm["epsilon"] == 0.0:
         prm["epsilon"] = 1.0
     prm["max_num"] = int(prm["max_num"]) * 2
+    return rng, (nd, origin, res, data, ctl, U, prm, start, goal, vel)
+
+
+def run_sequence(seed, dim, impls, rounds=4):
+    rng, (nd, origin, res, data, ctl, U, prm, start, goal, vel) = sequence_case(seed, dim)
     pls, maps_ = [], []
     for cm, cp, extra in impls:
         m = cm(origin, nd, data, res)
