@@ -38,7 +38,9 @@ extern "C" {
 #define MPLB_PLAN_QUEUE_EMPTY 3      /* "Priority queue is empty"              graph_search.h:157-161 */
 #define MPLB_PLAN_TRACEBACK_FAILED 4 /* recoverTraj returned false             graph_search.h:414-431,180-181 */
 #define MPLB_PLAN_START_IS_GOAL 5    /* Astar returned 0 before searching; plan() is true, traj untouched graph_search.h:44 */
-#define MPLB_PLAN_KEY_RANGE 7        /* a state left the packable lattice range (|vel| >> v_max, far outside map) */
+#define MPLB_PLAN_KEY_RANGE 7        /* a lattice int the reference cannot represent: round(x / 0.01 or 0.1) beyond int32 in the
+                                        start, or a successor outside the packable range (a derivative with an unset bound
+                                        beyond 100); a start merely outside the packable range is planned from */
 #define MPLB_PLAN_NOMEM 8            /* node arena exhausted at the largest tier that fits the device */
 
 /* Control::Control bit patterns, include/mpl_basis/control.h:10-20 */
@@ -329,6 +331,13 @@ int mplb_expand(mplb_planner *p, const mplb_waypoint *states, int n, mplb_prim_t
  * fast_delta (either may be NULL) receive the configuration's filter switch and guard band in cells.  HOST buffers. */
 int mplb_probe_samples(mplb_planner *p, const mplb_waypoint *states, int n, mplb_sample_probe *rows, int cap,
                        int32_t *use_fast, double *fast_delta);
+
+/* The configuration the search kernel would run for start waypoints of this control flag, on the planner's map and
+ * settings (parity artefact, read-only; shaped and yaw configurations included): key_bits = bits the packed lattice key
+ * spans, key_wide = 1 when that is more than 96 (hash-table slots then also compare the row's full second key word),
+ * use_fast = 1 when collision samples go through the filtered granule sampler, 0 when every control is sampled on the
+ * exact path.  Any output may be NULL.  Returns MPLB_OK, or the error planning with this configuration would return. */
+int mplb_planner_key_layout(mplb_planner *p, int32_t control, int32_t *key_bits, int32_t *key_wide, int32_t *use_fast);
 
 /* Correctly rounded sin/cos as the yaw branch evaluates them (primitive.h:520, env_map.h:125), computed on the device:
  * x, s, c are HOST arrays of n doubles, |x| < 2^20.  Parity artefact: tests compare it with the oracle and mpmath. */

@@ -61,6 +61,7 @@ SYMBOLS = {
     "mplb_get_open": (_I, [_VP, _VP, _I]),
     "mplb_expand": (_I, [_VP, _VP, _I, _VP]),
     "mplb_probe_samples": (_I, [_VP, _VP, _I, _VP, _I, _VP, _VP]),
+    "mplb_planner_key_layout": (_I, [_VP, _I, _VP, _VP, _VP]),
     "mplb_last_batch_stats": (_I, [_VP, _VP, _VP, _VP]),
     "mplb_comm_unique_id": (_I, [_VP]),
     "mplb_comm_create": (_I, [_VP, _I, _I, _VP]),

@@ -370,6 +370,7 @@ struct mplb_planner {
   DevBuf<double> d_U, d_ttab, d_Uyaw;
   DevBuf<int> d_toff, d_tcnt;
   int kfields = 0;
+  int key_bits = 0; /* bits the packed key spans, word 0's padding included */
 
   /* scratch */
   DevBuf<unsigned char> arena;
@@ -690,6 +691,7 @@ int build_cfg(mplb_planner *p, int control) {
     bitpos += bits;
   }
   c.key_wide = (bitpos > 96) ? 1 : 0;
+  p->key_bits = bitpos;
   p->kfields = c.nkey;
   p->cfg_control = control;
   p->cfg_map_version = m->version;
@@ -1608,10 +1610,17 @@ int mplb_get_nodes(mplb_planner *p, mplb_node *nodes, int cap) {
       for (int ax = 0; ax < c.dim; ax++) o.state[d * 3 + ax] = st[d * c.dim + ax];
     if (c.use_yaw) o.state[12] = st[c.dim * c.ord];
     o.g = hot[i].g; o.h = hot[i].h;
-    for (int f = 0; f < c.nkey; f++) {
-      unsigned long long wv = c.kword[f] ? rh->k1 : rh->k0;
-      unsigned long long v = (wv >> c.kshift[f]) & ((1ull << c.kbits[f]) - 1ull);
-      o.key[f] = (int)((long long)v + c.koff[f]);
+    if (rh->k0 == MPLB_KEY_OUT_OF_RANGE && rh->k1 == MPLB_KEY_OUT_OF_RANGE) { /* the start, outside the packable range */
+      for (int f = 0; f < c.nkey; f++) {
+        const int d = f < c.dim * c.ord ? f % c.ord : 1, ax = f / c.ord; /* field axis * ord + d; the yaw field last */
+        o.key[f] = mplb_ref::round_int(mplb_ref::ddiv(f < c.dim * c.ord ? st[d * c.dim + ax] : st[f], d == 0 ? 0.01 : 0.1));
+      }
+    } else {
+      for (int f = 0; f < c.nkey; f++) {
+        unsigned long long wv = c.kword[f] ? rh->k1 : rh->k0;
+        unsigned long long v = (wv >> c.kshift[f]) & ((1ull << c.kbits[f]) - 1ull);
+        o.key[f] = (int)((long long)v + c.koff[f]);
+      }
     }
     o.key[15] = c.nkey;
     o.opened = (hot[i].flags & 1) ? 1 : 0;
@@ -1718,6 +1727,17 @@ int mplb_probe_samples(mplb_planner *p, const mplb_waypoint *states, int n, mplb
   cudaFree(d_count);
   if (e != cudaSuccess) return fail(MPLB_ERR_CUDA, std::string("probe_samples: ") + cudaGetErrorString(e));
   return count;
+}
+
+int mplb_planner_key_layout(mplb_planner *p, int32_t control, int32_t *key_bits, int32_t *key_wide, int32_t *use_fast) {
+  if (!p) return fail(MPLB_ERR_ARG, "null argument");
+  if (set_device_of(p->device)) return fail(MPLB_ERR_CUDA, "cannot select the planner's device");
+  int rc = build_cfg(p, control);
+  if (rc != MPLB_OK) return rc;
+  if (key_bits) *key_bits = p->key_bits;
+  if (key_wide) *key_wide = p->cfg.key_wide;
+  if (use_fast) *use_fast = p->cfg.use_fast;
+  return MPLB_OK;
 }
 
 #ifdef MPLB_PHASE_TIMING

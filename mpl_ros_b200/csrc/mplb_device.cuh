@@ -229,6 +229,13 @@ __device__ __forceinline__ void lattice_ints(const double *st, int *ints) {
   }
 }
 
+/* Both words of the key of a state outside the packable range (an out-of-range start, a probed state).  No successor
+ * that the search probes packs to it, because the all-ones value of a field decodes to at least the field's upper end
+ * (koff + 2^kbits - 1 >= hi, build_cfg), and every such successor keeps one field below that end: its velocity, within
+ * v_max by validation (pr:449-475; control order >= 2 needs v_max > 0), or, for VEL controls, its positions, within
+ * 2 |u| dt of the map (a popped state has no valid successor unless its own position is inside the map, em:104). */
+#define MPLB_KEY_OUT_OF_RANGE (~0ull)
+
 /* Pack ints into the 128-bit node key (no parity hash); false when a field leaves its packable range. */
 template <int DIM, int ORD, int NF = DIM * ORD>
 __device__ __forceinline__ bool pack_key_nohash(const DevCfg &c, const int *ints, unsigned long long &k0, unsigned long long &k1) {

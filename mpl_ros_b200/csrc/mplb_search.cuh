@@ -639,6 +639,28 @@ __device__ __forceinline__ void lattice_ints_x(const DevCfg &c, const double *st
   lattice_ints<DIM, ORD>(st, ints);
   if (NS > DIM * ORD) ints[DIM * ORD] = c.use_yaw ? round_int(ddiv(st[DIM * ORD], 0.1)) : 0;
 }
+/* The reference's (int)std::round(x / q) of every key field of a state row is defined: the rounded quotient fits int32. */
+template <int DIM, int ORD, int NS>
+__device__ __forceinline__ bool lattice_ints_defined(const DevCfg &c, const double *st) {
+  bool ok = true;
+  for (int f = 0; f < NS; f++) {
+    if (f == DIM * ORD && !c.use_yaw) break;
+    const double r = mplb_ref::round_haz(ddiv(st[f], f < DIM ? 0.01 : 0.1));
+    ok = ok && r >= -2147483648.0 && r <= 2147483647.0;
+  }
+  return ok;
+}
+/* The state row of a waypoint (wp:22-58): the polynomial part, then the yaw slot of the cost-shaping / yaw kernels. */
+template <int DIM, int ORD, int NS>
+__device__ __forceinline__ void waypoint_state(const DevCfg &c, const mplb_waypoint &w, double *s) {
+  for (int ax = 0; ax < DIM; ax++) {
+    s[ax] = w.pos[ax];
+    if (ORD >= 2) s[DIM + ax] = w.vel[ax];
+    if (ORD >= 3) s[2 * DIM + ax] = w.acc[ax];
+    if (ORD >= 4) s[3 * DIM + ax] = w.jrk[ax];
+  }
+  if (NS > DIM * ORD) s[DIM * ORD] = c.use_yaw ? w.yaw : 0.0;
+}
 
 /* ---------------------------------------------------------------- phase B1: one lane per control (em:155-160,163-165) */
 template <int DIM, int ORD, class SM, class EBT>
@@ -957,6 +979,54 @@ __device__ __forceinline__ unsigned long long khash_of_ints(const int *ints, int
   return khash_final(h);
 }
 
+/* Start set-up (tid 0) of a start in S.cur whose lattice tuple lies outside the packable range: a derivative above its
+ * bound or an unwrapped yaw.  The reference plans from such a start.  Its tuple equals no successor's (validated
+ * successors lie inside the range), so it is pushed under the reserved key MPLB_KEY_OUT_OF_RANGE; otherwise as the
+ * kernel pushes an in-range start.  The pop loop hashes the lattice ints it unpacks from the current node's packed key;
+ * the hash seeds set here cancel what it unpacks from the reserved key and add the start's true tuple instead:
+ * (h ^ kh_true ^ kh_reserved) ^ kh_reserved = h ^ kh_true, and likewise for the sum.  A start whose (int)std::round of
+ * a field is undefined in the reference (the rounded quotient leaves int32) ends the plan with MPLB_PLAN_KEY_RANGE.
+ * Out of line: a cold path that must leave the search kernel's register allocation alone. */
+template <int DIM, int ORD, class SM>
+__device__ __noinline__ void start_out_of_range(const DevCfg &c, const BatchArgs &a, SM &S, int pid, NodeHot *hot, Slot *table,
+                                                unsigned char *rows, int *poplog) {
+  constexpr int NS = SM::NS;
+  if (!lattice_ints_defined<DIM, ORD, NS>(c, S.cur)) { S.status = MPLB_PLAN_KEY_RANGE; return; }
+  const int nk = (NS > DIM * ORD) ? c.nkey : NS;
+  int ints[NS], ur[NS];
+  lattice_ints_x<DIM, ORD, NS>(c, S.cur, ints);
+  const unsigned long long k = MPLB_KEY_OUT_OF_RANGE;
+  unpack_ints<NS>(c, k, k, ur);
+  const unsigned long long kh_true = khash_of_ints<NS>(ints, nk), kh_reserved = khash_of_ints<NS>(ur, nk);
+  /* eb:46-64: h = 0 on the goal's tuple, which only a comparison of the tuples shows here (a goal with this tuple is
+   * outside the range too); otherwise the heuristic gets a key that differs from the goal's */
+  const mplb_waypoint &gl = c.prior_on ? c.prior_goal : a.goals[pid];
+  bool at_goal = gl.control == c.control && gl.enable_t == 0;
+  if (at_goal) {
+    double gs[NS];
+    int gi[NS];
+    waypoint_state<DIM, ORD, NS>(c, gl, gs);
+    lattice_ints_x<DIM, ORD, NS>(c, gs, gi);
+    for (int f = 0; f < nk; f++) at_goal = at_goal && gi[f] == ints[f];
+  }
+  NodeHot n0;
+  n0.g = 0.0; n0.h = at_goal ? 0.0 : heuristic<DIM, ORD>(c, S, S.cur, ~S.gk0, S.gk1, 0); n0.pg = 0.0; n0.heap_pos = 0;
+  n0.action = -1; n0.flags = 3; n0.pad0 = 0;
+  hot[0] = n0;
+  int slot = table_insert_atomic(table, S.tsize, k, k, 0, 0.0, 0.0);
+  RowHdr *rh = reinterpret_cast<RowHdr *>(rows);
+  rh->k0 = k; rh->k1 = k; rh->parent = -1; rh->slot = slot; rh->pred_head = -1; rh->depth = 0;
+  double *rs = reinterpret_cast<double *>(rows + sizeof(RowHdr));
+  for (int f = 0; f < NS; f++) rs[f] = S.cur[f];
+  S.n_nodes = 1; S.n_heap = 0;
+  S.cur_node = 0; S.cur_g = 0.0; S.cur_tag = 0;
+  S.cur_k0 = k; S.cur_k1 = k;
+  S.pop_hash = 0xCBF29CE484222325ull ^ kh_true ^ kh_reserved;
+  S.closed_hash = kh_true - kh_reserved;
+  if (a.want_poplog) poplog[0] = 0;
+  S.pops = 1;
+}
+
 /* Generic serial relaxation of successors [i0, i1) in control order (lane 0 of warp 0): re-probes the table in
  * global memory, so it is correct under every hazard (duplicate siblings, slot collisions).  gs:79-143. */
 template <int DIM, int ORD, class SM>
@@ -1227,25 +1297,13 @@ astar_batch_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ Bat
       const mplb_waypoint &gl = c.prior_on ? c.prior_goal : gq;
       for (int ax = 0; ax < 3; ax++) { S.goal_pos[ax] = gl.pos[ax]; S.goal_vel[ax] = gl.vel[ax]; S.goal_acc[ax] = gl.acc[ax]; }
       double s0[NS];
-      for (int ax = 0; ax < DIM; ax++) {
-        s0[ax] = st.pos[ax];
-        if (ORD >= 2) s0[DIM + ax] = st.vel[ax];
-        if (ORD >= 3) s0[2 * DIM + ax] = st.acc[ax];
-        if (ORD >= 4) s0[3 * DIM + ax] = st.jrk[ax];
-      }
-      if (NS > NP) s0[NP] = c.use_yaw ? st.yaw : 0.0;
+      waypoint_state<DIM, ORD, NS>(c, st, s0);
       for (int f = 0; f < NS; f++) S.cur[f] = s0[f];
       /* goal lattice key: comparable only when the goal carries the same control flags (wp:92-125) */
       S.goal_key_ok = 0;
       if (gl.control == c.control && gl.enable_t == 0) {
         double gs[NS];
-        for (int ax = 0; ax < DIM; ax++) {
-          gs[ax] = gl.pos[ax];
-          if (ORD >= 2) gs[DIM + ax] = gl.vel[ax];
-          if (ORD >= 3) gs[2 * DIM + ax] = gl.acc[ax];
-          if (ORD >= 4) gs[3 * DIM + ax] = gl.jrk[ax];
-        }
-        if (NS > NP) gs[NP] = c.use_yaw ? gl.yaw : 0.0;
+        waypoint_state<DIM, ORD, NS>(c, gl, gs);
         int gi[NS];
         lattice_ints_x<DIM, ORD, NS>(c, gs, gi);
         S.goal_key_ok = pack_key_nohash<DIM, ORD, NS>(c, gi, S.gk0, S.gk1) ? 1 : 0;
@@ -1279,7 +1337,7 @@ astar_batch_kernel(const __grid_constant__ DevCfg c, const __grid_constant__ Bat
       int ints[NS];
       lattice_ints_x<DIM, ORD, NS>(c, S.cur, ints);
       unsigned long long k0, k1;
-      if (!pack_key_nohash<DIM, ORD, NS>(c, ints, k0, k1)) S.status = MPLB_PLAN_KEY_RANGE;
+      if (!pack_key_nohash<DIM, ORD, NS>(c, ints, k0, k1)) start_out_of_range<DIM, ORD>(c, a, S, pid, hot, table, rows, poplog);
       else {
         NodeHot n0;
         n0.g = 0.0; n0.h = heuristic<DIM, ORD>(c, S, S.cur, k0, k1, 0); n0.pg = 0.0; n0.heap_pos = 0; n0.action = -1;
@@ -1805,7 +1863,7 @@ __global__ void __launch_bounds__(MPLB_NT) expand_trace_kernel(const __grid_cons
       }
       int ints0[NS];
       lattice_ints<DIM, ORD>(E.st, ints0);
-      if (!pack_key_nohash<DIM, ORD>(c, ints0, E.pk0, E.pk1)) { E.pk0 = ~0ull; E.pk1 = ~0ull; } /* out-of-range state: nothing is its self-loop */
+      if (!pack_key_nohash<DIM, ORD>(c, ints0, E.pk0, E.pk1)) { E.pk0 = E.pk1 = MPLB_KEY_OUT_OF_RANGE; } /* out-of-range state: nothing is its self-loop */
       E.key_bad = 0;
     }
     __syncthreads();
@@ -1870,7 +1928,7 @@ __global__ void __launch_bounds__(MPLB_NT) probe_samples_kernel(const __grid_con
       }
       int ints0[DIM * ORD];
       lattice_ints<DIM, ORD>(E.st, ints0);
-      if (!pack_key_nohash<DIM, ORD>(c, ints0, E.pk0, E.pk1)) { E.pk0 = ~0ull; E.pk1 = ~0ull; }
+      if (!pack_key_nohash<DIM, ORD>(c, ints0, E.pk0, E.pk1)) { E.pk0 = E.pk1 = MPLB_KEY_OUT_OF_RANGE; }
     }
     __syncthreads();
     for (int i = tid; i < c.nU; i += MPLB_NT) expand_b1<DIM, ORD>(c, S, E, i);

@@ -626,6 +626,13 @@ class MapPlanner:
         rows = rows[np.lexsort((rows["k"], rows["control"], rows["state"]))]
         return rows, int(uf.value), float(fd.value)
 
+    def key_layout(self, control):
+        """The search configuration for start waypoints of `control` (mplb_planner_key_layout): dict of key_bits,
+        key_wide and use_fast.  Raises MplbError where planning with it would."""
+        kb, kw, uf = C.c_int32(), C.c_int32(), C.c_int32()
+        check(lib().mplb_planner_key_layout(self._h, int(control), C.byref(kb), C.byref(kw), C.byref(uf)))
+        return dict(key_bits=kb.value, key_wide=kw.value, use_fast=uf.value)
+
 
 class OccMapPlanner(MapPlanner):  # map_planner.h:122
     def __init__(self, verbose=False):

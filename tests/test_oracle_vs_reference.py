@@ -306,3 +306,33 @@ def test_map_ops_against_reference_sources():
     out[:, 1:, :][occ[:, :-1, :]] = 100
     out[:, :-1, :][occ[:, 1:, :]] = 100
     assert R.same("dilate", out.reshape(-1), rm.get_data)
+
+
+@pytest.mark.parametrize("group", ["wide", "exact", "out_of_range"])
+def test_key_edge_configurations(group):
+    """The configurations of tests/key_edge_cases.py that the GPU test compares with the oracle: unset dynamic bounds,
+    resolutions 0.045 .. 0.01, a map origin of 1.5e7 m at res 0.01, large-bound 3D SNP (wide lattice keys), and starts /
+    goals outside the packable key range (unwrapped yaws, derivatives above their bounds).  Every single plan of the GPU
+    test."""
+    import key_edge_cases as K
+    cases = {"wide": K.wide_cases, "exact": K.exact_cases, "out_of_range": K.oor_cases}[group]()
+    for name, branch, c, singles, _ in cases:
+        if c.map.res < 0.05 and c.dim == 3 and group == "exact" and "origin" not in name:
+            continue  # the 3D maps at res 0.045 only repeat what the 2D ones pin
+        op, rp = _pair(c.map, c.dim, c.params, c.U)
+        for sfl, gfl in singles:
+            s, g = _edge_waypoint(c, c.start, sfl), _edge_waypoint(c, c.goal, gfl)
+            _compare(op, rp, s, g, c.dim, c.control, c.U, (group, name, branch, c.dim, c.control, len(c.U), sorted(sfl.items()),
+                                                              sorted(gfl.items())), nodes=len(c.U) <= 32)
+
+
+def _edge_waypoint(c, pos, fields):
+    w = oracle.make_waypoints(1)
+    w["pos"][0, :c.dim] = pos
+    for k, v in fields.items():
+        if k == "yaw":
+            w["yaw"] = v
+        else:
+            w[k][0, :c.dim] = v
+    w["control"] = c.control
+    return w
