@@ -41,7 +41,10 @@ extern "C" {
 #define MPLB_PLAN_KEY_RANGE 7        /* a lattice int the reference cannot represent: round(x / 0.01 or 0.1) beyond int32 in the
                                         start, or a successor outside the packable range (a derivative with an unset bound
                                         beyond 100); a start merely outside the packable range is planned from */
-#define MPLB_PLAN_NOMEM 8            /* node arena exhausted at the largest tier that fits the device */
+#define MPLB_PLAN_NOMEM 8            /* node arena exhausted at the largest tier that fits the arena budget.  The record is fully
+                                        defined: n_seg 0, cost +inf, every counter, hash and device_ms 0, and the plan's action
+                                        row (when requested) all -1; segment states are not written.  A retained NOMEM plan
+                                        has no search state: mplb_get_nodes / _pop_log / _open fail with MPLB_ERR_STATE */
 
 /* Control::Control bit patterns, include/mpl_basis/control.h:10-20 */
 #define MPLB_CONTROL_VEL 1
@@ -155,10 +158,13 @@ enum mplb_param {
   MPLB_WYAW = 14,   /* setWyaw   :221 default 1.0 (env_base.h:372): weight of the heading cost env_map.h:121-128 */
   MPLB_MEM_FRACTION = 100, /* fraction of free device memory the search arenas may take (default 0.6) */
   MPLB_MAX_SLOTS = 101,    /* tuning: cap on concurrently resident plans (CTAs); 0 = all resident CTAs */
-  MPLB_EXACT_PREDS = 102   /* predecessor lists of graph_search.h:100-102 kept per node and resolved by recoverTraj with the
+  MPLB_EXACT_PREDS = 102,  /* predecessor lists of graph_search.h:100-102 kept per node and resolved by recoverTraj with the
                               final g values: -1 (default) = exactly where a running best predecessor could differ (epsilon > 1,
                               a prior-trajectory heuristic, VEL control with v_max below the control bound), 0 = never,
                               1 = always */
+  MPLB_ARENA_BYTES = 103   /* upper bound in bytes on the search-arena budget (0 = unset, the default): the budget is
+                              min(MPLB_MEM_FRACTION of the free memory, this).  Like MPLB_MEM_FRACTION it makes the next
+                              batch measure the budget again */
 };
 int mplb_planner_set_param(mplb_planner *p, int key, double value);
 /* setU (planner_base.h:246): n rows of udim doubles, udim = Dim, or Dim + 1 when the last entry is a yaw rate
@@ -346,6 +352,27 @@ int mplb_sincos_cr(const double *x, int n, double *s, double *c);
 /* Timing/diagnostics of the last batch on this planner: ms = device time of the search kernels (CUDA events on
  * the launch stream), launches = kernels launched, tiers = arena tiers used. Any pointer may be NULL. */
 int mplb_last_batch_stats(mplb_planner *p, double *kernel_ms, int32_t *launches, int32_t *tiers);
+
+/* One arena tier pass of the last A* batch (read-only diagnostics; DESIGN.md section 3, "Tiers").  A batch starts with
+ * every plan in one tier; plans that outgrow a tier's capacity run again from scratch in a larger one.  A pass that finds no
+ * tier fitting the arena budget launches nothing and marks its plans MPLB_PLAN_NOMEM (nomem = 1). */
+typedef struct mplb_tier_info {
+  int32_t cap;          /* node / heap capacity per plan */
+  int32_t slots;        /* plans resident at once (CTAs launched); for a NOMEM pass the slots the budget would have allowed */
+  int32_t n_work;       /* plans this pass ran (or marked NOMEM) */
+  int32_t n_overflow;   /* of those, plans that outgrew `cap` and go to the next pass */
+  int32_t hcap;         /* heap entries kept in shared memory per plan */
+  int32_t load_inv;     /* hash-table load factor bound 1 / load_inv */
+  int32_t tsize_max;    /* largest hash table per plan (slots) */
+  int32_t log_cap;      /* predecessor records per plan (0 unless in predecessor-log mode) */
+  int64_t stride_bytes; /* arena bytes per slot */
+  int32_t nomem;        /* 1: nothing launched, the pass only marked its plans MPLB_PLAN_NOMEM */
+  int32_t ordered;      /* 1: plans are taken from the longest-first work list, 0: in query order */
+  int32_t resident;     /* CTAs of the search kernel that fit the device at once */
+  int32_t reserved;
+} mplb_tier_info;
+/* Two-call pattern: returns the number of passes of the last batch and fills rows[0 .. min(count, cap)). */
+int mplb_last_batch_tiers(mplb_planner *p, mplb_tier_info *rows, int cap);
 
 /* ---- multi-GPU: one process per GPU, the batch sharded by query (query i -> rank i mod N), NCCL over NVLink.
  * Exactly two collectives exist on this path: one broadcast of the voxel grid per map and one gather of result records

@@ -25,7 +25,10 @@ NODE_DTYPE = np.dtype([("state", "f8", 13), ("g", "f8"), ("h", "f8"), ("key", "i
 LPA_NODE_DTYPE = np.dtype([("key", "i4", 16), ("state", "f8", 13), ("g", "f8"), ("rhs", "f8"), ("h", "f8"), ("opened", "i4"),
                            ("closed", "i4"), ("n_succ", "i4"), ("n_pred", "i4"), ("succ_hash", "u8"), ("pred_hash", "u8")], align=True)
 LPA_HEAP_DTYPE = np.dtype([("fval", "f8"), ("key_hash", "u8")], align=True)
-assert WAYPOINT_DTYPE.itemsize == 120 and RESULT_DTYPE.itemsize == 80
+TIER_DTYPE = np.dtype([("cap", "i4"), ("slots", "i4"), ("n_work", "i4"), ("n_overflow", "i4"), ("hcap", "i4"), ("load_inv", "i4"),
+                       ("tsize_max", "i4"), ("log_cap", "i4"), ("stride_bytes", "i8"), ("nomem", "i4"), ("ordered", "i4"),
+                       ("resident", "i4"), ("reserved", "i4")], align=True)
+assert WAYPOINT_DTYPE.itemsize == 120 and RESULT_DTYPE.itemsize == 80 and TIER_DTYPE.itemsize == 56
 
 # every symbol include/mplb.h declares: (restype, argtypes)
 _VP, _I, _D = C.c_void_p, C.c_int, C.c_double
@@ -63,6 +66,7 @@ SYMBOLS = {
     "mplb_probe_samples": (_I, [_VP, _VP, _I, _VP, _I, _VP, _VP]),
     "mplb_planner_key_layout": (_I, [_VP, _I, _VP, _VP, _VP]),
     "mplb_last_batch_stats": (_I, [_VP, _VP, _VP, _VP]),
+    "mplb_last_batch_tiers": (_I, [_VP, _VP, _I]),
     "mplb_comm_unique_id": (_I, [_VP]),
     "mplb_comm_create": (_I, [_VP, _I, _I, _VP]),
     "mplb_comm_destroy": (None, [_VP]),
@@ -101,7 +105,8 @@ SYMBOLS = {
 }
 
 PARAM = dict(v_max=0, a_max=1, j_max=2, yaw_max=3, dt=4, w=5, epsilon=6, max_num=7, tol_pos=8, tol_vel=9,
-             tol_acc=10, t_max=11, potential_weight=12, gradient_weight=13, wyaw=14, mem_fraction=100, max_slots=101, exact_preds=102)
+             tol_acc=10, t_max=11, potential_weight=12, gradient_weight=13, wyaw=14, mem_fraction=100, max_slots=101, exact_preds=102,
+             arena_bytes=103)
 
 _LIB = None
 

@@ -285,10 +285,20 @@ __global__ void k_serialize_traj(const __grid_constant__ MsgArgs a) {
   }
 }
 
-/* plans that fit no arena tier: their (internal overflow) status becomes MPLB_PLAN_NOMEM */
-__global__ void k_mark_status(mplb_result *results, const int *work, int n_work, int status) {
+/* plans that fit no arena tier get a complete MPLB_PLAN_NOMEM record: whatever the buffers held before (an earlier
+ * batch's record, the counters of an aborted smaller tier, a caller's stale data) must not show through */
+__global__ void k_mark_status(mplb_result *results, int *actions, int max_seg, const int *work, int n_work, int status) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n_work) results[work ? work[i] : i].status = status;
+  if (i >= n_work) return;
+  const int pid = work ? work[i] : i;
+  mplb_result r;
+  r.status = status; r.n_seg = 0; r.cost = __longlong_as_double(0x7ff0000000000000ll);
+  r.pops = 0; r.n_nodes = 0; r.n_open = 0; r.n_closed = 0;
+  r.n_prims = 0; r.n_samples = 0; r.n_valid = 0;
+  r.pop_hash = 0ull; r.closed_hash = 0ull; r.device_ms = 0.0;
+  results[pid] = r;
+  if (actions)
+    for (int k = 0; k < max_seg; k++) actions[(size_t)pid * max_seg + k] = -1;
 }
 
 __global__ void k_sincos_cr(const double *x, int n, double *s, double *c) {
@@ -338,7 +348,8 @@ struct mplb_planner {
   double mem_fraction = 0.6;
   int max_slots = 0; /* 0 = as many CTAs as are resident */
   int resident_sig = -1, resident_cached = 0, hcap_big_cached = 0, sm_count = 0;
-  size_t budget_bytes = 0; /* arena budget, measured at the first batch (reset by MPLB_MEM_FRACTION) */
+  size_t budget_bytes = 0; /* arena budget, measured at the first batch (reset by MPLB_MEM_FRACTION / MPLB_ARENA_BYTES) */
+  size_t arena_bytes = 0;  /* MPLB_ARENA_BYTES: upper bound on the budget, 0 = unset */
   std::vector<double> U; /* nU x 3 */
   std::vector<double> Uyaw; /* nU yaw rates when the rows have Dim + 1 entries (pr:217), else empty */
   int nU = 0;
@@ -387,8 +398,10 @@ struct mplb_planner {
   /* last batch */
   double last_ms = 0;
   int last_launches = 0, last_tiers = 0;
+  std::vector<mplb_tier_info> last_tier_rows; /* one per tier pass (mplb_last_batch_tiers) */
   /* retained single plan */
   bool retained = false;
+  bool ret_arena = false; /* the retained plan's search state is in the arena (false after MPLB_PLAN_NOMEM) */
   bool ret_lpa = false; /* the retained plan came from the LPA* unit: no A* arena behind the node getters */
   mplb_result ret_result;
   int ret_cap = 0, ret_ns = 0, ret_slot = 0;
@@ -825,12 +838,19 @@ int batch_launch_tier(mplb_planner *p, BatchRun &R) {
   int slots = std::min(R.n_work, R.resident);
   if (p->max_slots > 0) slots = std::min(slots, p->max_slots);
   if ((size_t)slots * L.stride > R.budget) slots = (int)(R.budget / L.stride);
+  mplb_tier_info row;
+  std::memset(&row, 0, sizeof(row));
+  row.cap = R.cap; row.slots = slots; row.n_work = R.n_work; row.load_inv = load_inv_of(R.cap); row.tsize_max = L.tsize_max;
+  row.log_cap = L.log_cap; row.stride_bytes = (int64_t)L.stride; row.ordered = R.identity ? 0 : 1; row.resident = R.resident;
   if (slots <= 0 || (long long)load_inv_of(R.cap) * ((long long)R.cap + c.nU) > (1ll << 30)) {
     /* nothing larger fits (or the table would pass 2^30 slots): the remaining plans report NOMEM.  In the first tier
      * the work list may be the identity (no id array was written), later tiers carry the overflow list. */
-    k_mark_status<<<(R.n_work + 255) / 256, 256, 0, s>>>(R.d_results, R.identity ? nullptr : p->d_work.p, R.n_work, MPLB_PLAN_NOMEM);
+    k_mark_status<<<(R.n_work + 255) / 256, 256, 0, s>>>(R.d_results, R.d_actions, R.max_seg, R.identity ? nullptr : p->d_work.p,
+                                                         R.n_work, MPLB_PLAN_NOMEM);
     g_launches++;
     CUDA_TRY(cudaGetLastError());
+    row.nomem = 1;
+    p->last_tier_rows.push_back(row);
     R.finished = true;
     return MPLB_OK;
   }
@@ -862,6 +882,8 @@ int batch_launch_tier(mplb_planner *p, BatchRun &R) {
   DISPATCH(c.dim, c.ord, c.nU, LAUNCH_CALL);
   if (rc != MPLB_OK) return rc;
   p->last_launches++; p->last_tiers++;
+  row.hcap = c.nU > 32 ? a.hcap : MPLB_HCAP; /* the |U| <= 32 instantiations keep a fixed top in their static shared memory */
+  p->last_tier_rows.push_back(row);
   R.slots = slots;
   R.n_this_tier = R.n_work;
   return MPLB_OK;
@@ -900,6 +922,7 @@ int run_batch_begin(mplb_planner *p, const mplb_waypoint *d_starts, const mplb_w
     size_t free_b = 0, total_b = 0;
     CUDA_TRY(cudaMemGetInfo(&free_b, &total_b));
     p->budget_bytes = (size_t)((double)(free_b + p->arena.n) * p->mem_fraction);
+    if (p->arena_bytes > 0) p->budget_bytes = std::min(p->budget_bytes, p->arena_bytes);
   }
 
   R = BatchRun();
@@ -915,6 +938,8 @@ int run_batch_begin(mplb_planner *p, const mplb_waypoint *d_starts, const mplb_w
   }
   R.cap = (int)std::min<long long>(cap, std::max<long long>(R.cap_bound, 1024));
   p->last_launches = 0; p->last_tiers = 0;
+  p->last_tier_rows.clear();
+  p->ret_arena = false;
   bool ev0_done = false;
   if (n > resident / 2 && n <= 65536) { /* longest-first order (scheduling only): see k_plan_keys */
     mplb_map *m = p->map;
@@ -973,9 +998,11 @@ int run_batch_end(mplb_planner *p) {
     int n_over = 0;
     CUDA_TRY(cudaMemcpyAsync(&n_over, p->d_ctrl.p + 1, sizeof(int), cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));
+    p->last_tier_rows.back().n_overflow = n_over;
     if (R.retain && R.n == 1 && n_over == 0) {
       p->ret_cap = R.cap; p->ret_ns = c.ns; p->ret_stride = R.L.stride; p->ret_off_state = R.L.off_rows; p->ret_row_bytes = R.L.row_bytes;
       p->ret_off_heap = R.L.off_heap; p->ret_off_poplog = R.L.off_poplog;
+      p->ret_arena = true;
     }
     if (n_over == 0) break;
     /* next tier: overflowed plans restart from scratch (the search is deterministic) with 8x the arena */
@@ -1276,6 +1303,11 @@ int mplb_planner_set_param(mplb_planner *p, int key, double v) {
     case MPLB_MEM_FRACTION:
       if (!(v > 0 && v <= 0.95)) return fail(MPLB_ERR_ARG, "mem fraction must be in (0, 0.95]");
       p->mem_fraction = v;
+      p->budget_bytes = 0;
+      break;
+    case MPLB_ARENA_BYTES:
+      if (!(v >= 0 && v < 9.0e18)) return fail(MPLB_ERR_ARG, "arena bytes must be >= 0 (0 = unset)");
+      p->arena_bytes = (size_t)v;
       p->budget_bytes = 0;
       break;
     case MPLB_MAX_SLOTS: p->max_slots = (int)v; break;
@@ -1588,9 +1620,16 @@ int mplb_get_seg_states(mplb_planner *p, double *states13, int cap) {
   return n;
 }
 
-int mplb_get_nodes(mplb_planner *p, mplb_node *nodes, int cap) {
+/* the node getters read the retained plan's arena slot: there is none after MPLB_PLAN_NOMEM (no tier ran it to the end) */
+static int check_retained_arena(mplb_planner *p) {
   if (!p || !p->retained) return fail(MPLB_ERR_STATE, "no retained plan");
   if (p->ret_lpa) return fail(MPLB_ERR_STATE, "the retained plan is an LPA* plan: use mplb_lpa_get_nodes / mplb_lpa_get_heap");
+  if (!p->ret_arena) return fail(MPLB_ERR_STATE, "the retained plan has no search state (MPLB_PLAN_NOMEM: no arena tier fit it)");
+  return MPLB_OK;
+}
+
+int mplb_get_nodes(mplb_planner *p, mplb_node *nodes, int cap) {
+  if (int rc = check_retained_arena(p)) return rc;
   int n = p->ret_result.n_nodes;
   if (!nodes || cap <= 0) return n;
   if (set_device_of(p->device)) return fail(MPLB_ERR_CUDA, "cannot select the planner's device");
@@ -1632,8 +1671,7 @@ int mplb_get_nodes(mplb_planner *p, mplb_node *nodes, int cap) {
 }
 
 int mplb_get_pop_log(mplb_planner *p, int32_t *node_ids, int cap) {
-  if (!p || !p->retained) return fail(MPLB_ERR_STATE, "no retained plan");
-  if (p->ret_lpa) return fail(MPLB_ERR_STATE, "the retained plan is an LPA* plan: use mplb_lpa_get_nodes / mplb_lpa_get_heap");
+  if (int rc = check_retained_arena(p)) return rc;
   int n = std::min(p->ret_result.pops, p->ret_cap);
   if (!node_ids || cap <= 0) return n;
   if (set_device_of(p->device)) return fail(MPLB_ERR_CUDA, "cannot select the planner's device");
@@ -1643,8 +1681,7 @@ int mplb_get_pop_log(mplb_planner *p, int32_t *node_ids, int cap) {
 }
 
 int mplb_get_open(mplb_planner *p, int32_t *node_ids, int cap) {
-  if (!p || !p->retained) return fail(MPLB_ERR_STATE, "no retained plan");
-  if (p->ret_lpa) return fail(MPLB_ERR_STATE, "the retained plan is an LPA* plan: use mplb_lpa_get_nodes / mplb_lpa_get_heap");
+  if (int rc = check_retained_arena(p)) return rc;
   int n = p->ret_result.n_open;
   if (!node_ids || cap <= 0) return n;
   if (set_device_of(p->device)) return fail(MPLB_ERR_CUDA, "cannot select the planner's device");
@@ -1830,6 +1867,13 @@ int mplb_last_batch_stats(mplb_planner *p, double *kernel_ms, int32_t *launches,
   if (launches) *launches = p->last_launches;
   if (tiers) *tiers = p->last_tiers;
   return MPLB_OK;
+}
+
+int mplb_last_batch_tiers(mplb_planner *p, mplb_tier_info *rows, int cap) {
+  if (!p) return fail(MPLB_ERR_ARG, "null planner");
+  const int n = (int)p->last_tier_rows.size();
+  for (int i = 0; i < n && i < cap && rows; i++) rows[i] = p->last_tier_rows[i];
+  return n;
 }
 
 

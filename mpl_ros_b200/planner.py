@@ -308,6 +308,7 @@ class MapPlanner:
 
     def setMemFraction(self, f): self._set("mem_fraction", f)
     def setMaxSlots(self, n): self._set("max_slots", n)
+    def setArenaBytes(self, n): self._set("arena_bytes", n)  # upper bound on the arena budget; 0 = unset
 
     def setDt(self, dt):
         self._set("dt", dt)
@@ -605,6 +606,14 @@ class MapPlanner:
         ms, l, t = C.c_double(), C.c_int32(), C.c_int32()
         check(lib().mplb_last_batch_stats(self._h, C.byref(ms), C.byref(l), C.byref(t)))
         return dict(kernel_ms=ms.value, launches=l.value, tiers=t.value)
+
+    def last_batch_tiers(self):
+        """One dict per arena tier pass of the last batch (mplb_tier_info: cap, slots, n_work, n_overflow, hcap, load_inv,
+        tsize_max, log_cap, stride_bytes, nomem, ordered, resident)."""
+        n = check(lib().mplb_last_batch_tiers(self._h, None, 0))
+        rows = np.zeros(max(n, 1), dtype=_lib.TIER_DTYPE)
+        check(lib().mplb_last_batch_tiers(self._h, ptr(rows), rows.size))
+        return [{k: int(r[k]) for k in _lib.TIER_DTYPE.names if k != "reserved"} for r in rows[:n]]
 
     def expand(self, states):
         """env_map::get_succ rows for arbitrary states (env_map.h:147-172): array [n, |U|] of trace records."""

@@ -21,6 +21,7 @@ TRACE_DTYPE = np.dtype([("verdict", "i4"), ("n", "i4"), ("n_tested", "i4"), ("bl
                         ("succ", "f8", 13), ("key", "i4", 16)], align=True)
 NODE_DTYPE = np.dtype([("state", "f8", 13), ("t", "f8"), ("g", "f8"), ("h", "f8"), ("key", "i4", 16),
                        ("opened", "i4"), ("closed", "i4")], align=True)
+HEAP_DTYPE = np.dtype([("key", "i4", 16), ("f", "f8"), ("key_hash", "u8")], align=True)
 
 
 def build(force=False):
@@ -62,6 +63,9 @@ def lib():
         L.orc_get_seg_states.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
         L.orc_get_nodes.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
         L.orc_get_pop_keys.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
+        L.orc_get_heap.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
+        L.orc_get_peaks.argtypes = [C.c_void_p, C.c_void_p]
+        L.orc_get_peaks.restype = None
         L.orc_get_succ_trace.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
         L.orc_plan_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
         L.orc_plan_batch_dyn.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
@@ -220,6 +224,19 @@ class OraclePlanner(LpaMixin):
         a = np.zeros((max(pops, 1), 16), dtype=np.int32)
         n = lib().orc_get_pop_keys(self.h, _ptr(a), a.shape[0])
         return a[:n]
+
+    def heap(self):
+        """pq_ of the last plan in its array order (HEAP_DTYPE: key rows, f, key hash)"""
+        n = lib().orc_get_heap(self.h, None, 0)
+        a = np.zeros(max(n, 1), dtype=HEAP_DTYPE)
+        n = lib().orc_get_heap(self.h, _ptr(a), a.size)
+        return a[:n]
+
+    def peaks(self):
+        """largest (nodes, heap, predecessor records) at the start of any expansion of the last plan (orc_get_peaks)"""
+        a = np.zeros(3, dtype=np.int64)
+        lib().orc_get_peaks(self.h, _ptr(a))
+        return dict(nodes=int(a[0]), heap=int(a[1]), records=int(a[2]))
 
     def succ_trace(self, curr):
         rows = np.zeros(self.nU, dtype=TRACE_DTYPE)

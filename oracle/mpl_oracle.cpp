@@ -595,6 +595,9 @@ struct Planner {
   std::vector<int> pop_order;
   std::vector<int> traj_actions;
   std::vector<int> traj_nodes;  // parent node of each segment
+  // largest hm_.size(), pq_.size() and predecessor-record count seen when an expansion starts (after its pop, before get_succ):
+  // the point where the CUDA kernel checks its arena capacity (orc_get_peaks)
+  int64_t peak_nodes = 0, peak_heap = 0, peak_records = 0;
   long long dbg_increase = 0, dbg_pred_total = 0, dbg_pred_hit = 0, dbg_pred_new = 0;
   int dbg_pred = -1, dbg_nodes_before = 0;  // decrease-key events (diagnostics, printed when ORC_DEBUG is set)
   orc_result last;
@@ -1226,6 +1229,7 @@ struct Planner {
 
   int plan(const WP &start, const WP &goal_) {
     nodes.clear(); hm.clear(); heap = Heap(); pop_order.clear(); traj_actions.clear(); traj_nodes.clear();
+    peak_nodes = peak_heap = peak_records = 0;
     std::memset(&last, 0, sizeof(last));
     last.cost = kInf;
     heap.nodes = &nodes;
@@ -1262,6 +1266,9 @@ struct Planner {
       heap.pop();
       dbg_pred = heap.empty() ? -1 : heap.top_node();
       dbg_nodes_before = (int)nodes.size();
+      peak_nodes = std::max<int64_t>(peak_nodes, (int64_t)nodes.size());
+      peak_heap = std::max<int64_t>(peak_heap, (int64_t)heap.q.size());
+      peak_records = std::max<int64_t>(peak_records, last.n_valid); /* one record per finite-cost edge so far (gs:100-102) */
       uint64_t kh = key_hash(nodes[curr].key);
       pop_hash = (pop_hash ^ kh) * 0x100000001B3ull;
       if (!nodes[curr].closed) { n_closed++; closed_hash += kh; }
@@ -1547,6 +1554,24 @@ int orc_get_nodes(void *pp, orc_node *out, int cap) {
     out[i].opened = nd.opened; out[i].closed = nd.closed;
   }
   return n;
+}
+int orc_get_heap(void *pp, orc_heap_entry *out, int cap) {
+  Planner *p = (Planner *)pp;
+  int n = (int)p->heap.q.size();
+  for (int i = 0; i < n && i < cap; i++) {
+    const Heap::Entry &e = p->heap.entries[p->heap.q[i]];
+    const Key &k = p->nodes[e.node].key;
+    std::memset(&out[i], 0, sizeof(orc_heap_entry));
+    for (int j = 0; j < k.n; j++) out[i].key[j] = k.v[j];
+    out[i].key[15] = k.n;
+    out[i].f = e.f;
+    out[i].key_hash = key_hash(k);
+  }
+  return n;
+}
+void orc_get_peaks(void *pp, int64_t *peaks3) {
+  Planner *p = (Planner *)pp;
+  peaks3[0] = p->peak_nodes; peaks3[1] = p->peak_heap; peaks3[2] = p->peak_records;
 }
 int orc_get_pop_keys(void *pp, int32_t *keys16, int cap) {
   Planner *p = (Planner *)pp;

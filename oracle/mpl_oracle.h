@@ -127,6 +127,19 @@ int orc_get_actions(void *p, int32_t *actions, int cap);                 /* retu
 int orc_get_seg_states(void *p, double *states13, int cap);              /* n_seg rows of 13 doubles (parent coord per segment) */
 int orc_get_nodes(void *p, orc_node *nodes, int cap);                    /* returns n_nodes (hash-map iteration, unordered) */
 int orc_get_pop_keys(void *p, int32_t *keys16, int cap);                 /* rows of 16 ints in pop order; returns pops */
+/* pq_ (Heap::q) in its array order; the same layout as the reference's d_ary_heap array as far as the stand-in
+ * oracle/shim/boost/heap/d_ary_heap.hpp mirrors Boost's (tests/test_oracle_vs_reference.py compares the two) */
+typedef struct orc_heap_entry {
+  int32_t key[16];   /* lattice ints of the entry's node, key[15] = count */
+  double f;          /* the stored priority g + eps * h at push / increase time */
+  uint64_t key_hash; /* of the key, as in pop_hash / closed_hash and orc_lpa_heap_entry */
+} orc_heap_entry;
+int orc_get_heap(void *p, orc_heap_entry *entries, int cap);             /* returns pq_.size() */
+/* Largest hm_.size(), pq_.size() and predecessor-record count (finite-cost edges so far) seen at the start of any
+ * expansion of the last orc_plan, i.e. after its pop and before get_succ — where the CUDA kernel checks its arena.  A plan
+ * overflows a tier of capacity C (|U| controls) exactly when nodes + |U| > C, heap + |U| + 1 > C, or, in predecessor-log
+ * mode, records + |U| > log_cap. */
+void orc_get_peaks(void *p, int64_t *peaks3);
 int orc_get_succ_trace(void *p, const orc_waypoint *curr, orc_prim_trace *rows, int cap); /* returns |U| */
 
 /* Batch: plans i = 0..n-1 striped over nthreads std::threads (one plan per thread at a time;

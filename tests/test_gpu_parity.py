@@ -307,8 +307,9 @@ def test_large_batch_uses_longest_first_order(name, dim, ctrl_u):
 
 def test_synthetic_boxes_jrk125_batch():
     """BASELINE configs[4] shape at test size: synthetic box map (seeded generator of SURVEY.md section 8d), jerk control,
-    |U| = 125, dt = 0.5, max_num bound.  Every plan here stops at MaxExpandStep with > 32 768 nodes, so the whole batch
-    goes through the second arena tier; counters and the pop-order hash must still match the oracle."""
+    |U| = 125, dt = 0.5, max_num bound.  Every plan here stops at MaxExpandStep with > 32 768 nodes; the MaxExpandStep
+    bound (300 * 125 + 2 * 125 + 64 = 37814 nodes) sizes the first and only arena tier, so no plan overflows.  Counters and
+    the pop-order hash must still match the oracle."""
     m = maps.synthetic_boxes(n=96, occupied_frac=0.2, seed=1, res=0.1)
     U = maps.make_U(2.0, 2, 3)
     params = dict(v_max=3.0, a_max=2.0, dt=0.5, max_num=300, tol_pos=0.5)
@@ -322,7 +323,9 @@ def test_synthetic_boxes_jrk125_batch():
     assert set(np.unique(ro["status"])) == {2} and ro["n_nodes"].max() > 32768
     for i in range(n):
         assert_results_equal(rg[i], ro[i], i)
-    assert pl.last_batch_stats()["tiers"] >= 1
+    assert pl.last_batch_stats()["tiers"] == 1
+    tiers = pl.last_batch_tiers()
+    assert len(tiers) == 1 and tiers[0]["cap"] == 37814 and tiers[0]["n_overflow"] == 0, tiers
 
 
 def test_full_bench_batch_parity():

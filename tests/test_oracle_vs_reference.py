@@ -17,6 +17,7 @@ import pytest
 
 import oracle
 from oracle import ref
+from oracle.lpa import LPA_HEAP_DTYPE
 from mpl_ros_b200 import maps
 from helpers import load_config
 import ref_record as R
@@ -173,6 +174,41 @@ def test_snp_2d_and_jrk_125_controls_3d():
     assert U5.shape[0] == 125
     op, rp = _pair(m, 3, dict(v_max=3.0, a_max=2.0, dt=0.5, max_num=400, tol_pos=0.5), U5)
     _compare(op, rp, _wp([5.5, 5.5, 0.5], 7), _wp([1.5, 1.5, 5.5], 7), 3, 7, U5, "JRK 125", nodes=False)
+
+
+@pytest.mark.parametrize("case", ["2D ACC eps 0", "2D VEL eps 2.5", "3D JRK 125", "3D ACC 27 eps 1"])
+def test_astar_heap_array_matches_reference(case):
+    """The oracle's priority queue after an A* plan (orc_get_heap, array order) against the reference's own pq_ iterated in
+    its array order (ref_harness.cpp's lpa_dump_heap, which an A* plan fills as well): stored f and key of every entry, on
+    deep heaps (hundreds to thousands of entries) left by MaxExpandStep stops.  The CUDA kernel's heap is compared with
+    orc_get_heap (tests/test_gpu_capacity.py), so this pins that comparison to the reference's sources -- but only as far
+    as the stand-in oracle/shim/boost/heap/d_ary_heap.hpp mirrors Boost's own array order, which is not checked here."""
+    corridor = load_config("corridor")
+    if case == "2D ACC eps 0":
+        m, dim, _, _, start, goal = corridor
+        U, ctl = maps.make_U(1.0, 2, 2), 3
+        params = dict(v_max=2.0, a_max=1.0, dt=1.0, tol_pos=0.5, epsilon=0.0, max_num=300)
+    elif case == "2D VEL eps 2.5":
+        m, dim, _, _, start, goal = corridor
+        U, ctl = maps.make_U(1.0, 2, 2), 1
+        params = dict(v_max=2.0, dt=0.5, tol_pos=0.5, epsilon=2.5, max_num=400)
+    elif case == "3D JRK 125":
+        m, dim, start, goal = maps.load_fixture("skir"), 3, [5.5, 5.5, 0.5], [1.5, 1.5, 5.5]
+        U, ctl = maps.make_U(2.0, 2, 3), 7
+        params = dict(v_max=3.0, a_max=2.0, dt=0.5, max_num=150, tol_pos=0.5)
+    else:
+        m, dim = maps.load_fixture("levine"), 3
+        S, G = maps.sample_queries(m, 1, seed=3)
+        start, goal = S[0], G[0]
+        U, ctl = maps.make_U(1.0, 1, 3), 3
+        params = dict(v_max=2.0, a_max=1.0, dt=1.0, tol_pos=0.5, max_num=400)
+    op, rp = _pair(m, dim, params, U)
+    ro, _ = _compare(op, rp, _wp(start, ctl), _wp(goal, ctl), dim, ctl, U, case, nodes=False)
+    heap = op.heap()
+    assert len(heap) == ro["n_open"] > 512, (case, ro["status"], len(heap))
+    ours = np.zeros(len(heap), dtype=LPA_HEAP_DTYPE)
+    ours["fval"], ours["key_hash"] = heap["f"], heap["key_hash"]
+    assert R.same(repr(case) + "/heap", ours, lambda: rp.lpa_heap()), case
 
 
 def test_goal_tolerances_and_weights():
