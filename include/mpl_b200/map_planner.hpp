@@ -397,9 +397,19 @@ class MapUtil {
     }
     return pns;
   }
+  /* isFree / isOccupied / isUnknown by coordinate (map_util.h:57-80): outside is none of them */
+  bool isFree(const Veci<Dim> &pn) { const int v = cell(pn); return v >= 0 && v < 100; }
+  bool isOccupied(const Veci<Dim> &pn) { return cell(pn) == 100; }
+  bool isUnknown(const Veci<Dim> &pn) { return cell(pn) == -1; }
   mplb_map *handle() const { return h_; }
 
  private:
+  int cell(const Veci<Dim> &pn) {
+    int32_t c[3] = {0, 0, 0}, v = std::numeric_limits<int32_t>::min();
+    for (int i = 0; i < Dim; i++) c[i] = pn(i);
+    if (h_) mplb_map_get_cells(h_, c, 1, &v);
+    return v;
+  }
   mplb_map *h_ = nullptr;
   decimal_t res_ = 0;
   Vecf<Dim> origin_d_;

@@ -412,6 +412,64 @@ int mplb_plan_batch_sharded_begin(mplb_planner *p, mplb_comm *c, const mplb_wayp
                                   int max_seg);
 int mplb_plan_batch_sharded_end(mplb_planner *p, mplb_comm *c, int n, mplb_result *results, int32_t *actions, int root);
 
+/* ---- VoxelGrid: the map builder of planning_ros_utils (include/planning_ros_utils/voxel_grid.h, src/mapping_utils/
+ * voxel_grid.cpp, cited vg:<line>), the map store of mpl_test_node/src/cloud_to_map.cpp and map_replanner_node.cpp.  Both of
+ * its int8 grids (map_ and inflated_map_) live on the device, x fastest, so a grid hands its map to an mplb_map without
+ * leaving the device.  Every member gives the reference's result bit for bit (DESIGN.md section 4.13).  Where the reference
+ * is undefined this library defines:
+ *   - a point whose quotient (pt - origin) / res is NaN or beyond int32 is outside (cast<int> is undefined there);
+ *   - clear_columns ignores a column outside the grid (clear(nx, ny), vg:31-33, does not check);
+ *   - allocate fails with MPLB_ERR_ARG and changes nothing when a truncated dimension or origin is negative (dimensions
+ *     only) or beyond int32, or when the grid would have more than 2^31 - 1 cells.
+ * Host point buffers are rows of 3 doubles; device point buffers are rows of 3 floats (fp32 = 1) or doubles, widened to
+ * double as the reference's vec_Vec3f does.  Calls are synchronous; `stream` (a cudaStream_t as void*, NULL = default)
+ * orders the reads of a caller's device buffers. */
+typedef struct mplb_voxel_grid mplb_voxel_grid;
+/* VoxelGrid(origin, dim, res) (vg:3-10): the empty grid, then allocate(dim, origin) */
+int mplb_voxel_grid_create(const double *origin, const double *dim_m, float res, mplb_voxel_grid **out);
+void mplb_voxel_grid_destroy(mplb_voxel_grid *g);
+/* allocate (vg:129-172): changed = 0 and nothing happens when the truncated geometry is unchanged; otherwise map_ is shifted
+ * by the integer origins and inflated_map_ is RESET to the shifted map_ (changed = 1).  changed may be NULL. */
+int mplb_voxel_grid_allocate(mplb_voxel_grid *g, const double *dim_m, const double *origin, int32_t *changed);
+/* dim_ (3 ints), origin_ (3 ints), origin_d_ (3 doubles), res_; any pointer may be NULL */
+int mplb_voxel_grid_get_info(const mplb_voxel_grid *g, int32_t *dim, int32_t *origin_i, double *origin_d, float *res);
+int mplb_voxel_grid_clear(mplb_voxel_grid *g); /* clear() (vg:12-16): both grids free */
+/* addCloud(pts) (vg:174-180): every inside point's cell of map_ becomes 100 */
+int mplb_voxel_grid_add_cloud(mplb_voxel_grid *g, const double *pts, int64_t n);
+int mplb_voxel_grid_add_cloud_device(mplb_voxel_grid *g, const void *d_pts, int64_t n, int fp32, void *stream);
+/* addCloud(pts, ns) (vg:182-199): ns = n_ns rows of 3 ints.  Returns the length of the new_obs list (>= 0) or an error;
+ * new_obs receives its first min(count, cap) cells as rows of 3 ints, in the reference's order.  A call emits a
+ * cell at most once, so count <= the grid's cell count and a buffer of that many rows always suffices. */
+int64_t mplb_voxel_grid_add_cloud_inflated(mplb_voxel_grid *g, const double *pts, int64_t n, const int32_t *ns, int n_ns,
+                                           int32_t *new_obs, int64_t cap);
+/* Same with device points (fp32 or fp64) and a device new_obs buffer; ns stays a host array */
+int64_t mplb_voxel_grid_add_cloud_inflated_device(mplb_voxel_grid *g, const void *d_pts, int64_t n, int fp32, const int32_t *ns,
+                                                  int n_ns, void *d_new_obs, int64_t cap, void *stream);
+/* Points per internal pass of the inflated insertion (0 = the default, 2^22 candidate cells per pass, about 134 MB of scratch).  The passes run
+ * one after another, which is exactly the sequential order, so this changes memory use and nothing else. */
+int mplb_voxel_grid_set_chunk_points(mplb_voxel_grid *g, int64_t points);
+int mplb_voxel_grid_decay(mplb_voxel_grid *g); /* decay() (vg:214-225): every cell > 0 of both grids is decremented */
+/* n cells (rows of 3 ints) of map_: column = 1 is fill(nx, ny) (vg:35-39, the z of a row is ignored), column = 0 is
+ * fill(nx, ny, nz) (vg:41-45); cells outside are ignored like the reference does */
+int mplb_voxel_grid_fill(mplb_voxel_grid *g, const int32_t *cells3, int n, int column);
+int mplb_voxel_grid_clear_columns(mplb_voxel_grid *g, const int32_t *cells3, int n); /* clear(nx, ny), vg:31-33, z ignored */
+/* getCloud (vg:18-29) / getLocalCloud (vg:47-69): centres of the cells > 0 of map_ / inflated_map_ (the local box), x outermost
+ * and z innermost.  Return the number of points and write the first min(count, cap) rows of 3 doubles. */
+int64_t mplb_voxel_grid_get_cloud(mplb_voxel_grid *g, double *pts, int64_t cap);
+int64_t mplb_voxel_grid_get_local_cloud(mplb_voxel_grid *g, const double *pos, const double *ori, const double *dim,
+                                        double *pts, int64_t cap);
+/* getMap / getInflatedMap (vg:71-127) data: 100 where the cell is > 0, else 0, x fastest; cap >= the cell count */
+int mplb_voxel_grid_get_map(mplb_voxel_grid *g, int inflated, int8_t *out, size_t cap);
+/* setMap(map_util, getMap()) without leaving the device: m must be 3D with the grid's dims, origin origin_d_ and res
+ * (double)res_ (MPLB_ERR_ARG otherwise).  Its cells are rewritten in place and its bricks rebuilt, as by mplb_map_set_data, so
+ * planners sharing m see the change. */
+int mplb_voxel_grid_write_map(mplb_voxel_grid *g, int inflated, mplb_map *m);
+/* a new mplb_map of the grid's geometry holding getMap / getInflatedMap, built device to device */
+int mplb_voxel_grid_create_map(mplb_voxel_grid *g, int inflated, mplb_map **out);
+/* MapUtil cell values for n cells (rows of 3 ints, the third ignored in 2D): the int8 value, or INT32_MIN outside the map
+ * (the material of isFree / isOccupied / isUnknown, map_util.h:44-80) */
+int mplb_map_get_cells(const mplb_map *m, const int32_t *cells3, int n, int32_t *values);
+
 #ifdef __cplusplus
 }
 #endif

@@ -102,6 +102,25 @@ SYMBOLS = {
                                                 _VP, C.c_size_t, _VP, _VP]),
     "mplb_serialize_trajectories": (_I, [_VP, _VP, _VP, _VP, _I, _I, _D, C.c_uint32, C.c_uint32, C.c_uint32, C.c_char_p,
                                          _VP, C.c_size_t, _VP]),
+    "mplb_voxel_grid_create": (_I, [_VP, _VP, C.c_float, _VP]),
+    "mplb_voxel_grid_destroy": (None, [_VP]),
+    "mplb_voxel_grid_allocate": (_I, [_VP, _VP, _VP, _VP]),
+    "mplb_voxel_grid_get_info": (_I, [_VP, _VP, _VP, _VP, _VP]),
+    "mplb_voxel_grid_clear": (_I, [_VP]),
+    "mplb_voxel_grid_add_cloud": (_I, [_VP, _VP, C.c_int64]),
+    "mplb_voxel_grid_add_cloud_device": (_I, [_VP, _VP, C.c_int64, _I, _VP]),
+    "mplb_voxel_grid_add_cloud_inflated": (C.c_int64, [_VP, _VP, C.c_int64, _VP, _I, _VP, C.c_int64]),
+    "mplb_voxel_grid_add_cloud_inflated_device": (C.c_int64, [_VP, _VP, C.c_int64, _I, _VP, _I, _VP, C.c_int64, _VP]),
+    "mplb_voxel_grid_set_chunk_points": (_I, [_VP, C.c_int64]),
+    "mplb_voxel_grid_decay": (_I, [_VP]),
+    "mplb_voxel_grid_fill": (_I, [_VP, _VP, _I, _I]),
+    "mplb_voxel_grid_clear_columns": (_I, [_VP, _VP, _I]),
+    "mplb_voxel_grid_get_cloud": (C.c_int64, [_VP, _VP, C.c_int64]),
+    "mplb_voxel_grid_get_local_cloud": (C.c_int64, [_VP, _VP, _VP, _VP, _VP, C.c_int64]),
+    "mplb_voxel_grid_get_map": (_I, [_VP, _I, _VP, C.c_size_t]),
+    "mplb_voxel_grid_write_map": (_I, [_VP, _I, _VP]),
+    "mplb_voxel_grid_create_map": (_I, [_VP, _I, _VP]),
+    "mplb_map_get_cells": (_I, [_VP, _VP, _I, _VP]),
 }
 
 PARAM = dict(v_max=0, a_max=1, j_max=2, yaw_max=3, dt=4, w=5, epsilon=6, max_num=7, tol_pos=8, tol_vel=9,

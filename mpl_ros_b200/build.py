@@ -14,6 +14,7 @@ UNITS = {
     "mplb.cu": [os.path.join(CSRC, h) for h in ("mplb_search.cuh", "mplb_device.cuh", "mplb_trig.cuh", "mplb_ref.h")] + _COMMON,
     "mplb_trajsolve.cu": [os.path.join(CSRC, "mplb_ref.h")] + _COMMON,
     "mplb_lpa.cu": [os.path.join(CSRC, h) for h in ("mplb_lpa_core.h", "mplb_ref.h")] + _COMMON,
+    "mplb_voxel.cu": [os.path.join(CSRC, "mplb_ref.h")] + _COMMON,
 }
 DEPS = [SRC] + UNITS["mplb.cu"]
 OUT = os.path.join(HERE, "libmplb.so")

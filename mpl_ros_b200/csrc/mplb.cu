@@ -1089,6 +1089,11 @@ int mplb_internal_planner_cfg(mplb_planner *p, MplbLpaHostCfg *o) {
   }
   return MPLB_OK;
 }
+void mplb_internal_map_view(mplb_map *m, MplbMapView *o) {
+  o->dim = m->dim; o->device = m->device; o->res = m->res; o->ncell = m->ncell; o->d_grid = m->d_grid;
+  for (int i = 0; i < 3; i++) { o->nd[i] = m->nd[i]; o->origin[i] = m->origin[i]; }
+}
+int mplb_internal_map_cells_changed(mplb_map *m, void *stream) { return m->rebuild_bricks((cudaStream_t)stream); }
 void mplb_internal_set_retained(mplb_planner *p, const mplb_result *res, const int *actions, const double *segs13, int n_seg) {
   p->ret_result = *res;
   p->ret_actions.assign(actions, actions + n_seg);

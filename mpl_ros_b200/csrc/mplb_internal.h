@@ -34,4 +34,18 @@ MPLB_HIDDEN void mplb_internal_set_retained(mplb_planner *p, const mplb_result *
 MPLB_HIDDEN int mplb_internal_lpa_enabled(mplb_planner *p);
 MPLB_HIDDEN int mplb_internal_lpa_plan(mplb_planner *p, const mplb_waypoint *start, const mplb_waypoint *goal, mplb_result *out);
 MPLB_HIDDEN void mplb_internal_lpa_drop(mplb_planner *p);
+
+/* ---- what the VoxelGrid unit (mplb_voxel.cu) needs from the map object of mplb.cu */
+struct mplb_map;
+struct MplbMapView {
+  int dim, device;
+  int nd[3];
+  double origin[3];
+  double res;
+  size_t ncell;
+  int8_t *d_grid; /* the map's int8 cells (x fastest) on `device` */
+};
+MPLB_HIDDEN void mplb_internal_map_view(mplb_map *m, MplbMapView *out);
+/* after d_grid was rewritten on `stream` (a cudaStream_t): rebuild the occupancy bit-bricks, as mplb_map_set_data does */
+MPLB_HIDDEN int mplb_internal_map_cells_changed(mplb_map *m, void *stream);
 #endif

@@ -255,6 +255,25 @@ MPLB_HD int ray_setup(int dim, double res, const double *p1, const double *p2, d
 /* point n on one axis: pt1 + step * n with step = diff * s (mu:121,126) */
 MPLB_HD double ray_point(double p1, double diff, double s, int n) { return dadd(p1, dmul(dmul(diff, s), (double)n)); }
 
+/* ------------------------------------------------------------------ VoxelGrid (planning_ros_utils voxel_grid.cpp, vg) */
+/* floatToInt (vg:201-203) on one axis: ((pt - origin_d_) / res_).cast<int>(), the float res_ widened to double and the
+ * quotient TRUNCATED toward zero (not MapUtil's rounding).  Returns false where cast<int> is undefined (a NaN quotient or
+ * one beyond int32); the grid treats such a point as outside. */
+MPLB_HD bool vg_float_to_cell(double pt, double origin_d, float res, int *n) {
+  const double q = ddiv(dsub(pt, origin_d), (double)res);
+  if (!(q > -2147483649.0 && q < 2147483648.0)) return false;
+#ifdef __CUDA_ARCH__
+  *n = __double2int_rz(q);
+#else
+  *n = (int)q;
+#endif
+  return true;
+}
+/* intToFloat (vg:205-207) on one axis: (n + 0.5) * res_ + origin_d_ in that order */
+MPLB_HD double vg_cell_to_float(int n, double origin_d, float res) {
+  return dadd(dmul(dadd((double)n, 0.5), (double)res), origin_d);
+}
+
 /* ------------------------------------------------------------------ lattice key hash (library and checker definition) */
 MPLB_HD unsigned long long khash_init() { return 0x243F6A8885A308D3ull; }
 MPLB_HD unsigned long long khash_step(unsigned long long h, int v) {

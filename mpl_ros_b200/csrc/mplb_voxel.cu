@@ -1,0 +1,662 @@
+/*
+ * mplb_voxel.cu — VoxelGrid on the GPU: the map builder of planning_ros_utils (include/planning_ros_utils/voxel_grid.h,
+ * src/mapping_utils/voxel_grid.cpp, cited vg:<line>) with both int8 grids resident in HBM, x fastest.
+ *
+ * Kernels (all memory bound):
+ *   k_vg_shift          allocate's copy of map_ into the new geometry (vg:139-160)
+ *   k_vg_add            addCloud(pts): one thread per point (vg:174-180); equal writes of 100 race benignly
+ *   k_vg_point_keys / k_vg_point_first / k_vg_cand_keys / k_vg_cand_first / k_vg_emit
+ *                       addCloud(pts, ns) (vg:182-199), whose output depends on the point order: per pass of consecutive
+ *                       points, (cell, point) and (cell, candidate id = i * |ns| + j) pairs are radix-sorted (stable, so equal
+ *                       cells keep id order) and the first claim of each cell wins; the winners are compacted in id order
+ *   k_vg_decay          decay (vg:214-225)
+ *   k_vg_fill / k_vg_clear_cols    fill / clear(nx, ny) (vg:31-45)
+ *   k_vg_row_count / k_vg_row_emit getCloud / getLocalCloud (vg:18-69): counts per (x, y) row, scan, ordered write
+ *   k_vg_binarize       getMap / getInflatedMap data (vg:71-127), also straight into an mplb_map's cells
+ * The sorts and scans are CUB's device-wide primitives.  Scratch scales with points x |ns| of one pass (about 32 B per
+ * candidate with CUB's sort storage) and with the x-y footprint for the clouds, never with the cell count (DESIGN.md 4.13).
+ */
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <climits>
+#include <cmath>
+#include <cstring>
+#include <string>
+#include <vector>
+
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
+
+#include "../../include/mplb.h"
+#include "mplb_internal.h"
+#include "mplb_ref.h"
+
+using namespace mplb_ref;
+
+namespace {
+
+#define VG_CUDA(expr)                                                                                                   \
+  do {                                                                                                                  \
+    cudaError_t e__ = (expr);                                                                                           \
+    if (e__ != cudaSuccess)                                                                                             \
+      return mplb_internal_fail(MPLB_ERR_CUDA, (std::string(#expr) + ": " + cudaGetErrorString(e__)).c_str());        \
+  } while (0)
+
+int vg_fail(int code, const char *msg) { return mplb_internal_fail(code, msg); }
+
+int set_device(int device) {
+  int cur = -1;
+  if (cudaGetDevice(&cur) != cudaSuccess) return -1;
+  if (cur != device && cudaSetDevice(device) != cudaSuccess) return -1;
+  return 0;
+}
+
+template <typename T>
+struct Buf { /* grow-only device buffer */
+  T *p = nullptr;
+  size_t n = 0;
+  cudaError_t reserve(size_t want) {
+    if (want <= n) return cudaSuccess;
+    if (p) cudaFree(p);
+    p = nullptr; n = 0;
+    cudaError_t e = cudaMalloc((void **)&p, want * sizeof(T));
+    if (e == cudaSuccess) n = want;
+    return e;
+  }
+  void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
+};
+
+/* geometry as the kernels see it */
+struct Geo {
+  int nd[3];
+  double origin_d[3];
+  float res;
+};
+
+int blocks_for(size_t n) { return (int)std::min<size_t>((n + 255) / 256, (size_t)148 * 32); }
+
+__device__ __forceinline__ double load_pt(const void *pts, int fp32, long long k) {
+  return fp32 ? (double)((const float *)pts)[k] : ((const double *)pts)[k];
+}
+/* floatToInt + isOutSide (vg:201-212): the linear x-fastest cell index, or -1 */
+__device__ __forceinline__ long long point_cell(const Geo &g, const void *pts, int fp32, long long i, int *c) {
+  for (int a = 0; a < 3; a++) {
+    if (!vg_float_to_cell(load_pt(pts, fp32, i * 3 + a), g.origin_d[a], g.res, &c[a])) return -1;
+    if (c[a] < 0 || c[a] >= g.nd[a]) return -1;
+  }
+  return (long long)c[0] + (long long)g.nd[0] * c[1] + (long long)g.nd[0] * g.nd[1] * c[2];
+}
+
+/* allocate (vg:139-160): new cell (l, w, h) takes old cell (l, w, h) + new_ori - ori when that is inside the old grid */
+__global__ void k_vg_shift(const int8_t *old_map, int ox, int oy, int oz, int8_t *out, int nx, int ny, int nz, int sx, int sy,
+                           int sz) {
+  const size_t total = (size_t)nx * ny * nz;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const long long l = (long long)(i % nx) + sx, w = (long long)((i / nx) % ny) + sy, h = (long long)(i / ((size_t)nx * ny)) + sz;
+    int8_t v = 0;
+    if (l >= 0 && l < ox && w >= 0 && w < oy && h >= 0 && h < oz) v = old_map[l + (long long)ox * w + (long long)ox * oy * h];
+    out[i] = v;
+  }
+}
+
+__global__ void k_vg_add(Geo g, const void *pts, int fp32, long long n, int8_t *map) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    int c[3];
+    const long long idx = point_cell(g, pts, fp32, i, c);
+    if (idx >= 0) map[idx] = 100;
+  }
+}
+
+/* one pass of addCloud(pts, ns) over points [i0, i0 + np): key = cell (ncell when outside), value = point */
+__global__ void k_vg_point_keys(Geo g, const void *pts, int fp32, long long i0, int np, unsigned ncell, unsigned *key, unsigned *val) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < np; i += gridDim.x * blockDim.x) {
+    int c[3];
+    const long long idx = point_cell(g, pts, fp32, i0 + i, c);
+    key[i] = idx >= 0 ? (unsigned)idx : ncell;
+    val[i] = (unsigned)i;
+  }
+}
+/* point i dilates iff it is inside, the first of the pass on its cell, and map_ there was not 100 when the pass began
+ * (earlier passes have written their cells; later points of this pass on the same cell see the 100 point i writes) */
+__global__ void k_vg_point_first(const unsigned *key, const unsigned *val, int np, unsigned ncell, const int8_t *map,
+                                 unsigned *pcell) {
+  for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < np; k += gridDim.x * blockDim.x) {
+    const unsigned c = key[k];
+    const bool first = c < ncell && (k == 0 || key[k - 1] != c);
+    pcell[val[k]] = (first && map[c] != 100) ? c : ncell; /* ncell: no dilation */
+  }
+}
+/* candidate id = i * n_ns + j: key = cell n_i + ns_j when point i dilates, that cell is inside and inflated_map_ there was not
+ * 100 when the pass began; ncell otherwise */
+__global__ void k_vg_cand_keys(const unsigned *pcell, int np, const int *ns, int n_ns, int nx, int ny, int nz, unsigned ncell,
+                               const int8_t *inf, unsigned *key, unsigned *val) {
+  const long long total = (long long)np * n_ns;
+  for (long long id = blockIdx.x * (long long)blockDim.x + threadIdx.x; id < total; id += (long long)gridDim.x * blockDim.x) {
+    const int i = (int)(id / n_ns), j = (int)(id % n_ns);
+    const unsigned c = pcell[i];
+    unsigned out = ncell;
+    if (c < ncell) {
+      const int x = (int)(c % (unsigned)nx) + ns[j * 3], y = (int)((c / (unsigned)nx) % (unsigned)ny) + ns[j * 3 + 1],
+                z = (int)(c / ((unsigned)nx * (unsigned)ny)) + ns[j * 3 + 2];
+      if (x >= 0 && x < nx && y >= 0 && y < ny && z >= 0 && z < nz) {
+        const unsigned c2 = (unsigned)x + (unsigned)nx * y + (unsigned)nx * ny * z;
+        if (inf[c2] != 100) out = c2;
+      }
+    }
+    key[id] = out;
+    val[id] = (unsigned)id;
+  }
+}
+/* the first candidate (lowest id) on each cell is emitted: flag[id] = 1 */
+__global__ void k_vg_cand_first(const unsigned *key, const unsigned *val, long long total, unsigned ncell, int *flag) {
+  for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < total; k += (long long)gridDim.x * blockDim.x) {
+    const unsigned c = key[k];
+    flag[val[k]] = (c < ncell && (k == 0 || key[k - 1] != c)) ? 1 : 0;
+  }
+}
+/* emitted candidates in id order: row base + pos[id] of new_obs (when < cap); inflated_map_ there becomes 100.  Then
+ * every inside point's cell of map_ becomes 100 (k_vg_add over the same points). */
+__global__ void k_vg_emit(const int *flag, const int *pos, const unsigned *pcell, long long total, const int *ns, int n_ns, int nx,
+                          int ny, int8_t *inf, int *out, long long base, long long cap) {
+  for (long long id = blockIdx.x * (long long)blockDim.x + threadIdx.x; id < total; id += (long long)gridDim.x * blockDim.x) {
+    if (!flag[id]) continue;
+    const int i = (int)(id / n_ns), j = (int)(id % n_ns);
+    const unsigned c = pcell[i];
+    const int x = (int)(c % (unsigned)nx) + ns[j * 3], y = (int)((c / (unsigned)nx) % (unsigned)ny) + ns[j * 3 + 1],
+              z = (int)(c / ((unsigned)nx * (unsigned)ny)) + ns[j * 3 + 2];
+    inf[(size_t)x + (size_t)nx * y + (size_t)nx * ny * z] = 100;
+    const long long r = base + pos[id];
+    if (r < cap) { out[r * 3] = x; out[r * 3 + 1] = y; out[r * 3 + 2] = z; }
+  }
+}
+
+__global__ void k_vg_decay(int8_t *a, int8_t *b, size_t n) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    if (a[i] > 0) a[i]--;
+    if (b[i] > 0) b[i]--;
+  }
+}
+
+/* fill(nx, ny) (column) / fill(nx, ny, nz) / clear(nx, ny) (value 0, column) on map_, cells outside ignored */
+__global__ void k_vg_fill(int8_t *map, const int *cells3, int n, int column, int8_t value, int nx, int ny, int nz) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const int x = cells3[k * 3], y = cells3[k * 3 + 1], z = cells3[k * 3 + 2];
+  if (x < 0 || x >= nx || y < 0 || y >= ny) return;
+  if (column) {
+    for (int h = 0; h < nz; h++) map[(size_t)x + (size_t)nx * y + (size_t)nx * ny * h] = value;
+  } else if (z >= 0 && z < nz) {
+    map[(size_t)x + (size_t)nx * y + (size_t)nx * ny * z] = value;
+  }
+}
+
+/* clouds over the box [lo, up): one thread per (x, y) with x fastest across threads (coalesced reads down each z);
+ * row r = (x - lo0) * by + (y - lo1) is the reference's x-outermost order */
+__global__ void k_vg_row_count(const int8_t *grid, int nx, int ny, int lo0, int lo1, int lo2, int bx, int by, int up2, int *cnt) {
+  const long long rows = (long long)bx * by;
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < rows; t += (long long)gridDim.x * blockDim.x) {
+    const int x = lo0 + (int)(t % bx), y = lo1 + (int)(t / bx);
+    int c = 0;
+    for (int z = lo2; z < up2; z++) c += grid[(size_t)x + (size_t)nx * y + (size_t)nx * ny * z] > 0;
+    cnt[(long long)(x - lo0) * by + (y - lo1)] = c;
+  }
+}
+__global__ void k_vg_row_emit(const int8_t *grid, Geo g, int lo0, int lo1, int lo2, int bx, int by, int up2, const int *off,
+                              double *out, long long cap) {
+  const int nx = g.nd[0], ny = g.nd[1];
+  const long long rows = (long long)bx * by;
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < rows; t += (long long)gridDim.x * blockDim.x) {
+    const int x = lo0 + (int)(t % bx), y = lo1 + (int)(t / bx);
+    long long r = off[(long long)(x - lo0) * by + (y - lo1)];
+    for (int z = lo2; z < up2 && r < cap; z++) {
+      if (grid[(size_t)x + (size_t)nx * y + (size_t)nx * ny * z] <= 0) continue;
+      out[r * 3] = vg_cell_to_float(x, g.origin_d[0], g.res);
+      out[r * 3 + 1] = vg_cell_to_float(y, g.origin_d[1], g.res);
+      out[r * 3 + 2] = vg_cell_to_float(z, g.origin_d[2], g.res);
+      r++;
+    }
+  }
+}
+
+__global__ void k_vg_binarize(const int8_t *src, int8_t *dst, size_t n) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+    dst[i] = src[i] > 0 ? 100 : 0;
+}
+
+__global__ void k_map_get_cells(const int8_t *grid, int dim, int nx, int ny, int nz, const int *cells3, int n, int *values) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const int x = cells3[k * 3], y = cells3[k * 3 + 1], z = dim == 3 ? cells3[k * 3 + 2] : 0;
+  values[k] = (x < 0 || x >= nx || y < 0 || y >= ny || z < 0 || z >= nz) ? INT_MIN
+                                                                          : (int)grid[(size_t)x + (size_t)nx * y + (size_t)nx * ny * z];
+}
+
+int key_bits(unsigned ncell) { /* radix-sort bits covering keys 0 .. ncell */
+  int b = 1;
+  while (b < 32 && (1ull << b) <= ncell) b++;
+  return b;
+}
+
+}  // namespace
+
+struct mplb_voxel_grid {
+  int dim[3] = {0, 0, 0};
+  int ori[3] = {0, 0, 0};
+  double origin_d[3] = {0, 0, 0};
+  float res = 0;
+  size_t ncell = 0;
+  int device = 0;
+  int8_t *d_map = nullptr, *d_inf = nullptr;
+  long long chunk_points = 0;
+  /* scratch of the inflated insertion and of the clouds */
+  Buf<unsigned> k0, k1, v0, v1, pcell;
+  Buf<int> flag, pos, ns, cells, rows, obs;
+  Buf<double> pts;
+  Buf<char> tmp;
+  Buf<int8_t> bytes;
+
+  Geo geo() const {
+    Geo g;
+    for (int i = 0; i < 3; i++) { g.nd[i] = dim[i]; g.origin_d[i] = origin_d[i]; }
+    g.res = res;
+    return g;
+  }
+  void release() {
+    if (d_map) cudaFree(d_map);
+    if (d_inf) cudaFree(d_inf);
+    d_map = d_inf = nullptr;
+    k0.release(); k1.release(); v0.release(); v1.release(); pcell.release(); flag.release(); pos.release(); ns.release();
+    obs.release(); cells.release(); rows.release(); pts.release(); tmp.release(); bytes.release();
+  }
+};
+
+namespace {
+
+int vg_allocate(mplb_voxel_grid *g, const double *dim_m, const double *origin, int32_t *changed) {
+  int nd[3], no[3];
+  for (int i = 0; i < 3; i++) { /* Vec3i new_dim(new_dim_d(i) / res_, ...), the float res_ widened (vg:130-131) */
+    const double qd = dim_m[i] / (double)g->res, qo = origin[i] / (double)g->res;
+    if (!(qd > -1.0 && qd < 2147483648.0)) return vg_fail(MPLB_ERR_ARG, "voxel grid dimension negative, NaN or beyond int32");
+    if (!(qo > -2147483649.0 && qo < 2147483648.0)) return vg_fail(MPLB_ERR_ARG, "voxel grid origin NaN or beyond int32");
+    nd[i] = (int)qd;
+    no[i] = (int)qo;
+  }
+  if (nd[2] == 0 && no[2] == 0) nd[2] = 1; /* vg:132 */
+  if (changed) *changed = 0;
+  if (nd[0] == g->dim[0] && nd[1] == g->dim[1] && nd[2] == g->dim[2] && no[0] == g->ori[0] && no[1] == g->ori[1] &&
+      no[2] == g->ori[2])
+    return MPLB_OK; /* vg:134-137 */
+  const size_t ncell = (size_t)nd[0] * nd[1] * nd[2];
+  if (ncell > 0x7fffffffull) return vg_fail(MPLB_ERR_ARG, "voxel grid of more than 2^31 - 1 cells");
+  int8_t *m = nullptr, *f = nullptr;
+  if (ncell) {
+    VG_CUDA(cudaMalloc((void **)&m, ncell));
+    cudaError_t e = cudaMalloc((void **)&f, ncell);
+    if (e != cudaSuccess) { cudaFree(m); return vg_fail(MPLB_ERR_CUDA, "cudaMalloc(voxel grid)"); }
+    k_vg_shift<<<blocks_for(ncell), 256>>>(g->d_map, g->dim[0], g->dim[1], g->dim[2], m, nd[0], nd[1], nd[2], no[0] - g->ori[0],
+                                            no[1] - g->ori[1], no[2] - g->ori[2]);
+    mplb_internal_count_launches(1);
+    e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpy(f, m, ncell, cudaMemcpyDeviceToDevice); /* inflated_map_ = new_map (vg:163-164) */
+    if (e != cudaSuccess) { cudaFree(m); cudaFree(f); return vg_fail(MPLB_ERR_CUDA, cudaGetErrorString(e)); }
+  }
+  if (g->d_map) cudaFree(g->d_map);
+  if (g->d_inf) cudaFree(g->d_inf);
+  g->d_map = m;
+  g->d_inf = f;
+  g->ncell = ncell;
+  for (int i = 0; i < 3; i++) { g->dim[i] = nd[i]; g->ori[i] = no[i]; g->origin_d[i] = origin[i]; }
+  if (changed) *changed = 1;
+  return MPLB_OK;
+}
+
+/* the CUB temporary storage of one call */
+template <class F>
+int with_tmp(mplb_voxel_grid *g, F f) {
+  size_t bytes = 0;
+  VG_CUDA(f((void *)nullptr, bytes));
+  VG_CUDA(g->tmp.reserve(std::max<size_t>(bytes, 1)));
+  VG_CUDA(f((void *)g->tmp.p, bytes));
+  return MPLB_OK;
+}
+
+/* addCloud(pts, ns) over device points; new_obs rows go to `out` (device) from row 0, the first `cap` of them */
+long long vg_add_inflated(mplb_voxel_grid *g, const void *d_pts, long long n, int fp32, const int *h_ns, int n_ns, int *out,
+                          long long cap, cudaStream_t s) {
+  if (n <= 0 || n_ns <= 0 || g->ncell == 0) {
+    if (n > 0 && g->ncell) { /* no offsets: only map_ changes */
+      k_vg_add<<<blocks_for((size_t)n), 256, 0, s>>>(g->geo(), d_pts, fp32, n, g->d_map);
+      mplb_internal_count_launches(1);
+      VG_CUDA(cudaGetLastError());
+      VG_CUDA(cudaStreamSynchronize(s));
+    }
+    return 0;
+  }
+  long long chunk = g->chunk_points > 0 ? g->chunk_points : std::max<long long>(1, (1ll << 22) / n_ns);
+  chunk = std::min<long long>(chunk, std::max<long long>(1, 0x7fffffffll / n_ns)); /* candidate ids stay below 2^31 */
+  chunk = std::min(chunk, n);
+  const long long cand = chunk * n_ns;
+  const unsigned ncell = (unsigned)g->ncell;
+  const int bits = key_bits(ncell);
+  VG_CUDA(g->ns.reserve((size_t)n_ns * 3));
+  VG_CUDA(cudaMemcpyAsync(g->ns.p, h_ns, (size_t)n_ns * 3 * sizeof(int), cudaMemcpyHostToDevice, s));
+  VG_CUDA(g->k0.reserve((size_t)cand)); VG_CUDA(g->k1.reserve((size_t)cand));
+  VG_CUDA(g->v0.reserve((size_t)cand)); VG_CUDA(g->v1.reserve((size_t)cand));
+  VG_CUDA(g->pcell.reserve((size_t)chunk));
+  VG_CUDA(g->flag.reserve((size_t)cand)); VG_CUDA(g->pos.reserve((size_t)cand));
+  const Geo geo = g->geo();
+  long long total = 0;
+  for (long long i0 = 0; i0 < n; i0 += chunk) {
+    const int np = (int)std::min(chunk, n - i0);
+    const long long nc = (long long)np * n_ns;
+    k_vg_point_keys<<<blocks_for(np), 256, 0, s>>>(geo, d_pts, fp32, i0, np, ncell, g->k0.p, g->v0.p);
+    VG_CUDA(cudaGetLastError());
+    int rc = with_tmp(g, [&](void *t, size_t &b) {
+      return cub::DeviceRadixSort::SortPairs(t, b, g->k0.p, g->k1.p, g->v0.p, g->v1.p, np, 0, bits, s);
+    });
+    if (rc) return rc;
+    k_vg_point_first<<<blocks_for(np), 256, 0, s>>>(g->k1.p, g->v1.p, np, ncell, g->d_map, g->pcell.p);
+    k_vg_cand_keys<<<blocks_for(nc), 256, 0, s>>>(g->pcell.p, np, g->ns.p, n_ns, g->dim[0], g->dim[1], g->dim[2], ncell, g->d_inf,
+                                                  g->k0.p, g->v0.p);
+    VG_CUDA(cudaGetLastError());
+    rc = with_tmp(g, [&](void *t, size_t &b) {
+      return cub::DeviceRadixSort::SortPairs(t, b, g->k0.p, g->k1.p, g->v0.p, g->v1.p, (int)nc, 0, bits, s);
+    });
+    if (rc) return rc;
+    k_vg_cand_first<<<blocks_for(nc), 256, 0, s>>>(g->k1.p, g->v1.p, nc, ncell, g->flag.p);
+    VG_CUDA(cudaGetLastError());
+    rc = with_tmp(g, [&](void *t, size_t &b) { return cub::DeviceScan::ExclusiveSum(t, b, g->flag.p, g->pos.p, (int)nc, s); });
+    if (rc) return rc;
+    k_vg_emit<<<blocks_for(nc), 256, 0, s>>>(g->flag.p, g->pos.p, g->pcell.p, nc, g->ns.p, n_ns, g->dim[0], g->dim[1], g->d_inf,
+                                             out, total, cap);
+    k_vg_add<<<blocks_for(np), 256, 0, s>>>(geo, (const char *)d_pts + i0 * 3 * (fp32 ? 4 : 8), fp32, np, g->d_map);
+    mplb_internal_count_launches(9);
+    VG_CUDA(cudaGetLastError());
+    int last[2];
+    VG_CUDA(cudaMemcpyAsync(&last[0], g->pos.p + nc - 1, sizeof(int), cudaMemcpyDeviceToHost, s));
+    VG_CUDA(cudaMemcpyAsync(&last[1], g->flag.p + nc - 1, sizeof(int), cudaMemcpyDeviceToHost, s));
+    VG_CUDA(cudaStreamSynchronize(s));
+    total += (long long)last[0] + last[1];
+  }
+  return total;
+}
+
+/* getCloud / getLocalCloud over the box [lo, up) of `grid` into device rows `out` */
+long long vg_cloud(mplb_voxel_grid *g, const int8_t *grid, const int *lo, const int *up, double *out, long long cap, cudaStream_t s) {
+  for (int i = 0; i < 3; i++) if (up[i] <= lo[i]) return 0;
+  const int bx = up[0] - lo[0], by = up[1] - lo[1];
+  const long long rows = (long long)bx * by;
+  VG_CUDA(g->rows.reserve((size_t)rows + 1));
+  VG_CUDA(g->flag.reserve((size_t)rows + 1));
+  k_vg_row_count<<<blocks_for(rows), 256, 0, s>>>(grid, g->dim[0], g->dim[1], lo[0], lo[1], lo[2], bx, by, up[2], g->flag.p);
+  VG_CUDA(cudaGetLastError());
+  VG_CUDA(cudaMemsetAsync(g->flag.p + rows, 0, sizeof(int), s));
+  int rc = with_tmp(g, [&](void *t, size_t &b) { return cub::DeviceScan::ExclusiveSum(t, b, g->flag.p, g->rows.p, (int)rows + 1, s); });
+  if (rc) return rc;
+  if (out && cap > 0) {
+    k_vg_row_emit<<<blocks_for(rows), 256, 0, s>>>(grid, g->geo(), lo[0], lo[1], lo[2], bx, by, up[2], g->rows.p, out, cap);
+    VG_CUDA(cudaGetLastError());
+  }
+  mplb_internal_count_launches(out && cap > 0 ? 3 : 2);
+  int total = 0;
+  VG_CUDA(cudaMemcpyAsync(&total, g->rows.p + rows, sizeof(int), cudaMemcpyDeviceToHost, s));
+  VG_CUDA(cudaStreamSynchronize(s));
+  return total;
+}
+
+long long host_cloud(mplb_voxel_grid *g, const int8_t *grid, const int *lo, const int *up, double *pts, long long cap) {
+  long long n = vg_cloud(g, grid, lo, up, nullptr, 0, 0);
+  if (n <= 0 || !pts || cap <= 0) return n;
+  const long long w = std::min(n, cap);
+  VG_CUDA(g->pts.reserve((size_t)w * 3));
+  long long rc = vg_cloud(g, grid, lo, up, g->pts.p, w, 0);
+  if (rc < 0) return rc;
+  VG_CUDA(cudaMemcpy(pts, g->pts.p, (size_t)w * 3 * sizeof(double), cudaMemcpyDeviceToHost));
+  return n;
+}
+
+int check_grid(const mplb_voxel_grid *g) {
+  if (!g) return vg_fail(MPLB_ERR_ARG, "null voxel grid");
+  if (set_device(g->device)) return vg_fail(MPLB_ERR_CUDA, "cannot select the voxel grid's device");
+  return MPLB_OK;
+}
+
+int upload_cells(mplb_voxel_grid *g, const int32_t *cells3, int n) {
+  VG_CUDA(g->cells.reserve((size_t)n * 3));
+  VG_CUDA(cudaMemcpy(g->cells.p, cells3, (size_t)n * 3 * sizeof(int), cudaMemcpyHostToDevice));
+  return MPLB_OK;
+}
+
+int vg_edit(mplb_voxel_grid *g, const int32_t *cells3, int n, int column, int8_t value) {
+  int rc = check_grid(g);
+  if (rc) return rc;
+  if (n < 0 || (n > 0 && !cells3)) return vg_fail(MPLB_ERR_ARG, "bad cell buffer");
+  if (n == 0 || !g->ncell) return MPLB_OK;
+  rc = upload_cells(g, cells3, n);
+  if (rc) return rc;
+  k_vg_fill<<<(n + 255) / 256, 256>>>(g->d_map, g->cells.p, n, column, value, g->dim[0], g->dim[1], g->dim[2]);
+  mplb_internal_count_launches(1);
+  VG_CUDA(cudaGetLastError());
+  VG_CUDA(cudaDeviceSynchronize());
+  return MPLB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int mplb_voxel_grid_create(const double *origin, const double *dim_m, float res, mplb_voxel_grid **out) {
+  if (!origin || !dim_m || !out) return vg_fail(MPLB_ERR_ARG, "null argument");
+  if (!(res > 0) || !std::isfinite(res)) return vg_fail(MPLB_ERR_ARG, "voxel grid resolution must be finite and > 0");
+  mplb_voxel_grid *g = new mplb_voxel_grid();
+  g->res = res;
+  if (cudaGetDevice(&g->device) != cudaSuccess) { delete g; return vg_fail(MPLB_ERR_CUDA, "no CUDA device (libmplb has no CPU path)"); }
+  int rc = vg_allocate(g, dim_m, origin, nullptr);
+  if (rc == MPLB_OK && cudaDeviceSynchronize() != cudaSuccess) rc = vg_fail(MPLB_ERR_CUDA, "voxel grid allocation");
+  if (rc != MPLB_OK) { g->release(); delete g; return rc; }
+  *out = g;
+  return MPLB_OK;
+}
+
+void mplb_voxel_grid_destroy(mplb_voxel_grid *g) {
+  if (!g) return;
+  set_device(g->device);
+  g->release();
+  delete g;
+}
+
+int mplb_voxel_grid_allocate(mplb_voxel_grid *g, const double *dim_m, const double *origin, int32_t *changed) {
+  int rc = check_grid(g);
+  if (rc) return rc;
+  if (!dim_m || !origin) return vg_fail(MPLB_ERR_ARG, "null argument");
+  rc = vg_allocate(g, dim_m, origin, changed);
+  if (rc) return rc;
+  VG_CUDA(cudaDeviceSynchronize());
+  return MPLB_OK;
+}
+
+int mplb_voxel_grid_get_info(const mplb_voxel_grid *g, int32_t *dim, int32_t *origin_i, double *origin_d, float *res) {
+  if (!g) return vg_fail(MPLB_ERR_ARG, "null voxel grid");
+  for (int i = 0; i < 3; i++) {
+    if (dim) dim[i] = g->dim[i];
+    if (origin_i) origin_i[i] = g->ori[i];
+    if (origin_d) origin_d[i] = g->origin_d[i];
+  }
+  if (res) *res = g->res;
+  return MPLB_OK;
+}
+
+int mplb_voxel_grid_clear(mplb_voxel_grid *g) {
+  int rc = check_grid(g);
+  if (rc) return rc;
+  if (!g->ncell) return MPLB_OK;
+  VG_CUDA(cudaMemset(g->d_map, 0, g->ncell));
+  VG_CUDA(cudaMemset(g->d_inf, 0, g->ncell));
+  VG_CUDA(cudaDeviceSynchronize());
+  return MPLB_OK;
+}
+
+int mplb_voxel_grid_add_cloud_device(mplb_voxel_grid *g, const void *d_pts, int64_t n, int fp32, void *stream) {
+  int rc = check_grid(g);
+  if (rc) return rc;
+  if (n < 0 || (n > 0 && !d_pts)) return vg_fail(MPLB_ERR_ARG, "bad point buffer");
+  if (n == 0 || !g->ncell) return MPLB_OK;
+  cudaStream_t s = (cudaStream_t)stream;
+  k_vg_add<<<blocks_for((size_t)n), 256, 0, s>>>(g->geo(), d_pts, fp32 ? 1 : 0, n, g->d_map);
+  mplb_internal_count_launches(1);
+  VG_CUDA(cudaGetLastError());
+  VG_CUDA(cudaStreamSynchronize(s));
+  return MPLB_OK;
+}
+
+int mplb_voxel_grid_add_cloud(mplb_voxel_grid *g, const double *pts, int64_t n) {
+  int rc = check_grid(g);
+  if (rc) return rc;
+  if (n < 0 || (n > 0 && !pts)) return vg_fail(MPLB_ERR_ARG, "bad point buffer");
+  if (n == 0 || !g->ncell) return MPLB_OK;
+  VG_CUDA(g->pts.reserve((size_t)n * 3));
+  VG_CUDA(cudaMemcpy(g->pts.p, pts, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice));
+  return mplb_voxel_grid_add_cloud_device(g, g->pts.p, n, 0, nullptr);
+}
+
+int64_t mplb_voxel_grid_add_cloud_inflated_device(mplb_voxel_grid *g, const void *d_pts, int64_t n, int fp32, const int32_t *ns,
+                                                  int n_ns, void *d_new_obs, int64_t cap, void *stream) {
+  int rc = check_grid(g);
+  if (rc) return rc;
+  if (n < 0 || (n > 0 && !d_pts) || n_ns < 0 || (n_ns > 0 && !ns) || cap < 0 || (cap > 0 && !d_new_obs))
+    return vg_fail(MPLB_ERR_ARG, "bad argument");
+  return vg_add_inflated(g, d_pts, n, fp32 ? 1 : 0, ns, n_ns, (int *)d_new_obs, cap, (cudaStream_t)stream);
+}
+
+int64_t mplb_voxel_grid_add_cloud_inflated(mplb_voxel_grid *g, const double *pts, int64_t n, const int32_t *ns, int n_ns,
+                                           int32_t *new_obs, int64_t cap) {
+  int rc = check_grid(g);
+  if (rc) return rc;
+  if (n < 0 || (n > 0 && !pts) || n_ns < 0 || (n_ns > 0 && !ns) || cap < 0 || (cap > 0 && !new_obs))
+    return vg_fail(MPLB_ERR_ARG, "bad argument");
+  if (n == 0) return 0;
+  cap = std::min<int64_t>(cap, (int64_t)g->ncell); /* one call emits a cell at most once: the rows past ncell stay unused */
+  VG_CUDA(g->pts.reserve((size_t)n * 3));
+  VG_CUDA(cudaMemcpy(g->pts.p, pts, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice));
+  if (cap > 0) VG_CUDA(g->obs.reserve((size_t)cap * 3));
+  const long long count = vg_add_inflated(g, g->pts.p, n, 0, ns, n_ns, g->obs.p, cap, 0);
+  if (count > 0 && cap > 0)
+    VG_CUDA(cudaMemcpy(new_obs, g->obs.p, (size_t)std::min<long long>(count, cap) * 3 * sizeof(int), cudaMemcpyDeviceToHost));
+  return count;
+}
+
+int mplb_voxel_grid_set_chunk_points(mplb_voxel_grid *g, int64_t points) {
+  if (!g || points < 0) return vg_fail(MPLB_ERR_ARG, "bad argument");
+  g->chunk_points = points;
+  return MPLB_OK;
+}
+
+int mplb_voxel_grid_decay(mplb_voxel_grid *g) {
+  int rc = check_grid(g);
+  if (rc) return rc;
+  if (!g->ncell) return MPLB_OK;
+  k_vg_decay<<<blocks_for(g->ncell), 256>>>(g->d_map, g->d_inf, g->ncell);
+  mplb_internal_count_launches(1);
+  VG_CUDA(cudaGetLastError());
+  VG_CUDA(cudaDeviceSynchronize());
+  return MPLB_OK;
+}
+
+int mplb_voxel_grid_fill(mplb_voxel_grid *g, const int32_t *cells3, int n, int column) {
+  return vg_edit(g, cells3, n, column ? 1 : 0, 100);
+}
+
+int mplb_voxel_grid_clear_columns(mplb_voxel_grid *g, const int32_t *cells3, int n) { return vg_edit(g, cells3, n, 1, 0); }
+
+int64_t mplb_voxel_grid_get_cloud(mplb_voxel_grid *g, double *pts, int64_t cap) {
+  int rc = check_grid(g);
+  if (rc) return rc;
+  if (cap < 0) return vg_fail(MPLB_ERR_ARG, "negative capacity");
+  const int lo[3] = {0, 0, 0};
+  return host_cloud(g, g->d_map, lo, g->dim, pts, cap);
+}
+
+int64_t mplb_voxel_grid_get_local_cloud(mplb_voxel_grid *g, const double *pos, const double *ori, const double *dim, double *pts,
+                                        int64_t cap) {
+  int rc = check_grid(g);
+  if (rc) return rc;
+  if (!pos || !ori || !dim || cap < 0) return vg_fail(MPLB_ERR_ARG, "bad argument");
+  int lo[3], up[3];
+  for (int i = 0; i < 3; i++) { /* vg:49-55: floatToInt(pos + ori) clamped >= 0, floatToInt(pos + ori + dim) clamped <= dim_ */
+    const double a = pos[i] + ori[i], b = a + dim[i];
+    int na, nb;
+    if (!vg_float_to_cell(a, g->origin_d[i], g->res, &na)) na = INT_MIN; /* cast<int> undefined: x86's INT_MIN */
+    if (!vg_float_to_cell(b, g->origin_d[i], g->res, &nb)) nb = INT_MIN;
+    lo[i] = na < 0 ? 0 : na;
+    up[i] = nb > g->dim[i] ? g->dim[i] : nb;
+  }
+  return host_cloud(g, g->d_inf, lo, up, pts, cap);
+}
+
+int mplb_voxel_grid_get_map(mplb_voxel_grid *g, int inflated, int8_t *out, size_t cap) {
+  int rc = check_grid(g);
+  if (rc) return rc;
+  if (!out && g->ncell) return vg_fail(MPLB_ERR_ARG, "null output");
+  if (cap < g->ncell) return vg_fail(MPLB_ERR_ARG, "output buffer smaller than the grid");
+  if (!g->ncell) return MPLB_OK;
+  VG_CUDA(g->bytes.reserve(g->ncell));
+  k_vg_binarize<<<blocks_for(g->ncell), 256>>>(inflated ? g->d_inf : g->d_map, g->bytes.p, g->ncell);
+  mplb_internal_count_launches(1);
+  VG_CUDA(cudaGetLastError());
+  VG_CUDA(cudaMemcpy(out, g->bytes.p, g->ncell, cudaMemcpyDeviceToHost));
+  return MPLB_OK;
+}
+
+int mplb_voxel_grid_write_map(mplb_voxel_grid *g, int inflated, mplb_map *m) {
+  int rc = check_grid(g);
+  if (rc) return rc;
+  if (!m) return vg_fail(MPLB_ERR_ARG, "null map");
+  MplbMapView v;
+  mplb_internal_map_view(m, &v);
+  if (v.dim != 3 || v.device != g->device || v.res != (double)g->res)
+    return vg_fail(MPLB_ERR_ARG, "map is not 3D on the grid's device with the grid's resolution");
+  for (int i = 0; i < 3; i++)
+    if (v.nd[i] != g->dim[i] || v.origin[i] != g->origin_d[i]) return vg_fail(MPLB_ERR_ARG, "map geometry differs from the grid's");
+  k_vg_binarize<<<blocks_for(g->ncell), 256>>>(inflated ? g->d_inf : g->d_map, v.d_grid, g->ncell);
+  mplb_internal_count_launches(1);
+  VG_CUDA(cudaGetLastError());
+  rc = mplb_internal_map_cells_changed(m, nullptr);
+  if (rc) return rc;
+  VG_CUDA(cudaDeviceSynchronize());
+  return MPLB_OK;
+}
+
+int mplb_voxel_grid_create_map(mplb_voxel_grid *g, int inflated, mplb_map **out) {
+  int rc = check_grid(g);
+  if (rc) return rc;
+  if (!out) return vg_fail(MPLB_ERR_ARG, "null argument");
+  if (!g->ncell) return vg_fail(MPLB_ERR_ARG, "the grid has no cells");
+  VG_CUDA(g->bytes.reserve(g->ncell));
+  k_vg_binarize<<<blocks_for(g->ncell), 256>>>(inflated ? g->d_inf : g->d_map, g->bytes.p, g->ncell);
+  mplb_internal_count_launches(1);
+  VG_CUDA(cudaGetLastError());
+  return mplb_map_create_from_device(3, g->dim, g->origin_d, (double)g->res, g->bytes.p, nullptr, out);
+}
+
+int mplb_map_get_cells(const mplb_map *m, const int32_t *cells3, int n, int32_t *values) {
+  if (!m || n < 0 || (n > 0 && (!cells3 || !values))) return vg_fail(MPLB_ERR_ARG, "bad argument");
+  if (n == 0) return MPLB_OK;
+  MplbMapView v;
+  mplb_internal_map_view(const_cast<mplb_map *>(m), &v);
+  if (set_device(v.device)) return vg_fail(MPLB_ERR_CUDA, "cannot select the map's device");
+  int *d = nullptr;
+  VG_CUDA(cudaMalloc((void **)&d, (size_t)n * 4 * sizeof(int)));
+  cudaError_t e = cudaMemcpy(d, cells3, (size_t)n * 3 * sizeof(int), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) {
+    k_map_get_cells<<<(n + 255) / 256, 256>>>(v.d_grid, v.dim, v.nd[0], v.nd[1], v.nd[2], d, n, d + (size_t)n * 3);
+    mplb_internal_count_launches(1);
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaMemcpy(values, d + (size_t)n * 3, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost);
+  cudaFree(d);
+  if (e != cudaSuccess) return vg_fail(MPLB_ERR_CUDA, cudaGetErrorString(e));
+  return MPLB_OK;
+}
+
+}  // extern "C"

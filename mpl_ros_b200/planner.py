@@ -171,6 +171,16 @@ class MapUtil:
         c3[:, :c.shape[1]] = c
         check(lib().mplb_map_set_cells(self._h, ptr(c3), len(c3), int(value)))
 
+    def getCells(self, cells):
+        """Values of cells (rows of Dim ints) as int32, INT32_MIN outside: the material of isFree / isOccupied
+        (map_util.h:44-80)."""
+        c = np.asarray(cells, dtype=np.int32).reshape(len(cells), -1)
+        c3 = np.zeros((len(c), 3), dtype=np.int32)
+        c3[:, :c.shape[1]] = c
+        out = np.zeros(max(len(c3), 1), dtype=np.int32)
+        check(lib().mplb_map_get_cells(self._h, ptr(c3), len(c3), ptr(out)))
+        return out[:len(c3)]
+
     def freeUnknown(self):  # map_util.h:259-276
         check(lib().mplb_map_free_unknown(self._h))
 
