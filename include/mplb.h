@@ -162,10 +162,17 @@ enum mplb_param {
                               final g values: -1 (default) = exactly where a running best predecessor could differ (epsilon > 1,
                               a prior-trajectory heuristic, VEL control with v_max below the control bound), 0 = never,
                               1 = always */
-  MPLB_ARENA_BYTES = 103   /* upper bound in bytes on the search-arena budget (0 = unset, the default): the budget is
+  MPLB_ARENA_BYTES = 103,  /* upper bound in bytes on the search-arena budget (0 = unset, the default): the budget is
                               min(MPLB_MEM_FRACTION of the free memory, this).  Like MPLB_MEM_FRACTION it makes the next
                               batch measure the budget again */
+  MPLB_LPA_INIT_NODES = 104, /* LPA*: node capacity of a session when it allocates (first plan, and the first plan after
+                                mplb_planner_reset); default 65 536.  Any whole number in [MPLB_LPA_MIN_CAP, MPLB_LPA_MAX_INIT],
+                                powers of two or not; other values fail with MPLB_ERR_ARG.  The arrays double when a plan
+                                needs more, so this decides when growth happens and nothing else: results do not depend on it */
+  MPLB_LPA_INIT_PREDS = 105  /* LPA*: predecessor-record capacity at allocation; default 2^20; same range and rules */
 };
+#define MPLB_LPA_MIN_CAP 128        /* smallest accepted MPLB_LPA_INIT_NODES / MPLB_LPA_INIT_PREDS */
+#define MPLB_LPA_MAX_INIT (1 << 28) /* largest accepted one */
 int mplb_planner_set_param(mplb_planner *p, int key, double value);
 /* setU (planner_base.h:246): n rows of udim doubles, udim = Dim, or Dim + 1 when the last entry is a yaw rate
  * (primitive.h:217); the row index is the action id. */
@@ -302,7 +309,9 @@ int mplb_get_linked_nodes(mplb_planner *p, double *pts3, int cap);
 int mplb_update_blocked_nodes(mplb_planner *p, const int32_t *cells3, int n);
 int mplb_update_cleared_nodes(mplb_planner *p, const int32_t *cells3, int n);
 /* Many replanners in one launch (one CTA each; e.g. one per robot): every planner must have LPA* enabled and live on the same
- * device; entry i behaves exactly like mplb_plan(planners[i], &starts[i], &goals[i], &results[i]). */
+ * device; entry i behaves exactly like mplb_plan(planners[i], &starts[i], &goals[i], &results[i]), including the retained
+ * trajectory of any length for mplb_get_actions / mplb_get_seg_states.  A session that has to grow stops before the pop that
+ * could overflow; the host doubles its arrays and relaunches the batch, in which finished sessions return at once. */
 int mplb_lpa_plan_batch(mplb_planner **planners, int n, const mplb_waypoint *starts, const mplb_waypoint *goals, mplb_result *results);
 /* State dumps (parity artefacts and getCloseSet / getOpenSet material): hm_ in iteration order, pq_ in its array order,
  * best_child_ (start .. goal).  Two-call pattern: cap = 0 returns the size. */
@@ -320,6 +329,15 @@ typedef struct mplb_lpa_heap_entry {
 int mplb_lpa_get_nodes(mplb_planner *p, mplb_lpa_node *out, int cap);
 int mplb_lpa_get_heap(mplb_planner *p, mplb_lpa_heap_entry *out, int cap);
 int mplb_lpa_get_best_child(mplb_planner *p, mplb_lpa_node *out, int cap); /* succ_hash / pred_hash left 0 */
+/* Capacity of the session's device arrays (read-only diagnostics; DESIGN.md section 4.12).  cap_nodes: node records (and the
+ * successor, iteration-order, heap and best_child_ arrays sized with them); cap_pred: predecessor records; tsize: key-table slots;
+ * n_nodes_physical: node records in use, including those a getSubStateSpace dropped from hm_ (they keep their id and are reset
+ * in place if a plan reaches their key again), so it never shrinks between resets; grows: doublings since the session allocated
+ * (before a pop that could overflow, or before a plan whose new start node would not fit).  getSubStateSpace may also enlarge
+ * the predecessor pool to (records its sweep can append) + |U|, which is not a power of two and is not counted in grows.  Any
+ * pointer may be NULL.  Fails with MPLB_ERR_STATE before the first LPA* plan. */
+int mplb_lpa_get_capacity(mplb_planner *p, int32_t *cap_nodes, int32_t *cap_pred, int32_t *tsize, int32_t *n_nodes_physical,
+                          int32_t *grows);
 
 /* Result getters of the retained single plan (two-call pattern: pass cap = 0 to get the size). */
 int mplb_get_actions(mplb_planner *p, int32_t *actions, int cap);      /* returns n_seg; recoverTraj graph_search.h:369-455 */

@@ -93,6 +93,7 @@ SYMBOLS = {
     "mplb_lpa_get_nodes": (_I, [_VP, _VP, _I]),
     "mplb_lpa_get_heap": (_I, [_VP, _VP, _I]),
     "mplb_lpa_get_best_child": (_I, [_VP, _VP, _I]),
+    "mplb_lpa_get_capacity": (_I, [_VP, _VP, _VP, _VP, _VP, _VP]),
     "mplb_refine_trajectories_device": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _VP, _VP, _VP]),
     "mplb_refine_trajectories": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _VP, _VP]),
     "mplb_traj_solve_batch": (_I, [_I, _I, _I, _I, _VP, _VP, _VP, _VP, _VP]),
@@ -125,7 +126,7 @@ SYMBOLS = {
 
 PARAM = dict(v_max=0, a_max=1, j_max=2, yaw_max=3, dt=4, w=5, epsilon=6, max_num=7, tol_pos=8, tol_vel=9,
              tol_acc=10, t_max=11, potential_weight=12, gradient_weight=13, wyaw=14, mem_fraction=100, max_slots=101, exact_preds=102,
-             arena_bytes=103)
+             arena_bytes=103, lpa_init_nodes=104, lpa_init_preds=105)
 
 _LIB = None
 

@@ -350,6 +350,7 @@ struct mplb_planner {
   int resident_sig = -1, resident_cached = 0, hcap_big_cached = 0, sm_count = 0;
   size_t budget_bytes = 0; /* arena budget, measured at the first batch (reset by MPLB_MEM_FRACTION / MPLB_ARENA_BYTES) */
   size_t arena_bytes = 0;  /* MPLB_ARENA_BYTES: upper bound on the budget, 0 = unset */
+  int lpa_init_nodes = 1 << 16, lpa_init_preds = 1 << 20; /* MPLB_LPA_INIT_NODES / _PREDS: LPA* array sizes at allocation */
   std::vector<double> U; /* nU x 3 */
   std::vector<double> Uyaw; /* nU yaw rates when the rows have Dim + 1 entries (pr:217), else empty */
   int nU = 0;
@@ -1078,6 +1079,7 @@ int mplb_internal_planner_cfg(mplb_planner *p, MplbLpaHostCfg *o) {
   o->dim = p->dim; o->nU = p->nU; o->max_num = p->max_num; o->device = p->device; o->verbose = p->verbose;
   o->v_max = p->v_max; o->a_max = p->a_max; o->j_max = p->j_max; o->dt = p->dt; o->w = p->w; o->eps = p->eps;
   o->tol_pos = p->tol_pos; o->tol_vel = p->tol_vel; o->tol_acc = p->tol_acc;
+  o->lpa_init_nodes = p->lpa_init_nodes; o->lpa_init_preds = p->lpa_init_preds;
   o->U = p->U.data();
   o->Uyaw = p->Uyaw.empty() ? nullptr : p->Uyaw.data();
   o->shaped = (p->pot_cells != 0 || !p->h_region.empty() || p->prior_nseg != 0 || !p->Uyaw.empty()) ? 1 : 0;
@@ -1314,6 +1316,12 @@ int mplb_planner_set_param(mplb_planner *p, int key, double v) {
       if (!(v >= 0 && v < 9.0e18)) return fail(MPLB_ERR_ARG, "arena bytes must be >= 0 (0 = unset)");
       p->arena_bytes = (size_t)v;
       p->budget_bytes = 0;
+      break;
+    case MPLB_LPA_INIT_NODES:
+    case MPLB_LPA_INIT_PREDS:
+      if (!(v >= MPLB_LPA_MIN_CAP && v <= MPLB_LPA_MAX_INIT && v == std::floor(v)))
+        return fail(MPLB_ERR_ARG, "LPA* initial sizes must be whole numbers in [MPLB_LPA_MIN_CAP, MPLB_LPA_MAX_INIT]");
+      (key == MPLB_LPA_INIT_NODES ? p->lpa_init_nodes : p->lpa_init_preds) = (int)v;
       break;
     case MPLB_MAX_SLOTS: p->max_slots = (int)v; break;
     case MPLB_EXACT_PREDS: p->exact_preds = (int)v; break;

@@ -19,6 +19,7 @@ struct mplb_waypoint;
 struct MplbLpaHostCfg {
   int dim, nU, max_num, device, verbose, has_map;
   int shaped; /* potential map / search region / prior trajectory / yaw controls installed: not available under LPA* */
+  int lpa_init_nodes, lpa_init_preds; /* MPLB_LPA_INIT_NODES / MPLB_LPA_INIT_PREDS */
   double v_max, a_max, j_max, dt, w, eps, tol_pos, tol_vel, tol_acc;
   int nd[3];
   double origin[3];

@@ -16,8 +16,10 @@
  *   k_lpa_link_count / k_lpa_link_scan / k_lpa_link_fill    the voxel -> edge table in insertion order (count, scan, fill)
  *   k_lpa_match       one thread per link against the changed voxels;  k_lpa_apply  sort + increaseCost / decreaseCost
  *   k_lpa_rehash      node table rebuild after the host grew the arrays
- * Capacity: arrays start at 65 536 nodes and double when a pop could overflow them (the kernel stops BEFORE the pop and the
- * host grows and resumes), so a search is never truncated.
+ *   k_lpa_traj        the whole trajectory of a plan longer than the batch's per-plan rows (action ids, parent coords)
+ * Capacity: arrays start at MPLB_LPA_INIT_NODES nodes / MPLB_LPA_INIT_PREDS predecessor records (65 536 / 2^20 by default) and
+ * double when a pop could overflow them (the kernel stops BEFORE the pop and the host grows and resumes), or before a plan whose
+ * start node would not fit (plan_begin may create one node and has no stop of its own), so a search is never truncated.
  */
 #include <cuda_runtime.h>
 
@@ -206,6 +208,15 @@ __global__ void k_lpa_rehash(Ctx *ctxs) {
   Ctx x = ctxs[0];
   for (int i = 0; i < x.h->n_nodes; i++) table_insert(x, i);
 }
+/* the trajectory recover() left in traj_act / best, for plans longer than k_lpa_plan's rows: one thread per segment */
+__global__ void k_lpa_traj(const Ctx *ctx, int n_seg, int *acts, double *segs) {
+  const Ctx &x = *ctx;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_seg) return;
+  acts[i] = x.traj_act[i];
+  const Node &pn = x.nodes[x.best[i]];
+  for (int k = 0; k < 13; k++) segs[(size_t)i * 13 + k] = pn.st[k];
+}
 
 /* ------------------------------------------------------------------ host side */
 template <typename T>
@@ -224,6 +235,8 @@ struct Buf {
   }
   void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
 };
+template <typename T>
+struct TmpBuf : Buf<T> { ~TmpBuf() { this->release(); } }; /* freed on every return path */
 
 struct Session {
   bool on = false;
@@ -245,6 +258,8 @@ struct Session {
   Buf<mplb_result> res;
   Buf<int> acts;
   int cap_nodes = 0, cap_pred = 0, tsize = 0, nU = 0, n_links_host = 0;
+  int init_nodes = 1 << 16, init_pred = 1 << 20; /* MPLB_LPA_INIT_NODES / _PREDS, read at every plan, used when allocating */
+  int grows = 0;                                 /* doublings since the arrays were allocated */
   bool have_links = false;
   void release() {
     d_ctx.release(); d_hdr.release(); nodes.release(); succ.release(); preds.release(); table.release(); order.release();
@@ -345,6 +360,7 @@ int refresh_cfg(mplb_planner *p, Session *s, int control) {
   LPA_CUDA(cudaSetDevice(hc.device));
   s->device = hc.device;
   s->nU = hc.nU;
+  s->init_nodes = hc.lpa_init_nodes; s->init_pred = hc.lpa_init_preds;
   LPA_CUDA(s->U.grow((size_t)hc.nU * 3, 0));
   LPA_CUDA(cudaMemcpy(s->U.p, hc.U, (size_t)hc.nU * 3 * sizeof(double), cudaMemcpyHostToDevice));
   Cfg &c = s->h.cfg;
@@ -358,11 +374,17 @@ int refresh_cfg(mplb_planner *p, Session *s, int control) {
 
 int reset_state(Session *s) { /* PlannerBase::reset: the next plan starts a new StateSpace (and may use other controls) */
   s->release();
-  s->cap_nodes = 0; s->cap_pred = 0; s->tsize = 0; s->nU = 0; s->n_links_host = 0;
+  s->cap_nodes = 0; s->cap_pred = 0; s->tsize = 0; s->nU = 0; s->n_links_host = 0; s->grows = 0;
   s->have_links = false;
   s->control = 0;
   std::memset(&s->h, 0, sizeof(s->h));
   return MPLB_OK;
+}
+
+/* double every array of the session, keeping its contents */
+int grow_session(Session *s) {
+  s->grows++;
+  return ensure_capacity(s, s->cap_nodes * 2, s->cap_pred * 2, true);
 }
 
 int plan_sessions(std::vector<mplb_planner *> &ps, const mplb_waypoint *starts, const mplb_waypoint *goals, mplb_result *results) {
@@ -376,13 +398,19 @@ int plan_sessions(std::vector<mplb_planner *> &ps, const mplb_waypoint *starts, 
     if (rc) return rc;
     if (i > 0 && s->device != ss[0]->device) return mplb_internal_fail(MPLB_ERR_ARG, "LPA* batch: all planners must live on one device");
     s->control = starts[i].control;
-    if (s->cap_nodes == 0) { rc = ensure_capacity(s, 1 << 16, 1 << 20, false); if (rc) return rc; }
+    if (s->cap_nodes == 0) { rc = ensure_capacity(s, s->init_nodes, s->init_pred, false); if (rc) return rc; }
     else { rc = upload_ctx(s); if (rc) return rc; }
+    /* room for the start node: plan_begin creates it when its key is new, and a pop may have filled the arrays exactly
+       (the pop-time check keeps only n_nodes <= cap_nodes; n_order and n_heap never exceed n_nodes) */
+    Hdr hd;
+    rc = read_hdr(s, &hd);
+    if (rc) return rc;
+    if (hd.n_nodes + 1 > s->cap_nodes) { rc = grow_session(s); if (rc) return rc; }
   }
   /* the batch's contexts, contiguous */
   Session *lead = ss[0];
-  const int max_seg = 4096;
-  struct CtxArray : Buf<Ctx> { ~CtxArray() { release(); } } ctxs; /* freed on every return path */
+  const int max_seg = 4096; /* per-plan trajectory rows of the launch; longer trajectories are gathered after it */
+  TmpBuf<Ctx> ctxs;
   LPA_CUDA(ctxs.grow(n, 0));
   for (int i = 0; i < n; i++) LPA_CUDA(cudaMemcpy(ctxs.p + i, &ss[i]->h, sizeof(Ctx), cudaMemcpyHostToDevice));
   LPA_CUDA(lead->wps.grow((size_t)2 * n, 0));
@@ -392,6 +420,7 @@ int plan_sessions(std::vector<mplb_planner *> &ps, const mplb_waypoint *starts, 
   LPA_CUDA(cudaMemcpy(lead->wps.p, starts, (size_t)n * sizeof(mplb_waypoint), cudaMemcpyHostToDevice));
   LPA_CUDA(cudaMemcpy(lead->wps.p + n, goals, (size_t)n * sizeof(mplb_waypoint), cudaMemcpyHostToDevice));
   for (int i = 0; i < n; i++) { Hdr hd; int rc = read_hdr(ss[i], &hd); if (rc) return rc; hd.resume = 0; hd.status = 0; rc = write_hdr(ss[i], hd); if (rc) return rc; }
+  /* every round doubles the arrays of the sessions that stopped, so 64 rounds cannot run out before int capacities do */
   for (int round = 0; round < 64; round++) {
     k_lpa_plan<<<n, 32>>>(ctxs.p, lead->wps.p, lead->wps.p + n, lead->res.p, lead->acts.p, lead->segs.p, max_seg);
     mplb_internal_count_launches(1);
@@ -404,7 +433,7 @@ int plan_sessions(std::vector<mplb_planner *> &ps, const mplb_waypoint *starts, 
       int rc = read_hdr(ss[i], &hd);
       if (rc) return rc;
       if (hd.status == LPA_NEED_GROW) { /* stopped before a pop that could overflow: double and resume */
-        rc = ensure_capacity(ss[i], ss[i]->cap_nodes * 2, ss[i]->cap_pred * 2, true);
+        rc = grow_session(ss[i]);
         if (rc) return rc;
         LPA_CUDA(cudaMemcpy(ctxs.p + i, &ss[i]->h, sizeof(Ctx), cudaMemcpyHostToDevice));
         again = true;
@@ -418,11 +447,24 @@ int plan_sessions(std::vector<mplb_planner *> &ps, const mplb_waypoint *starts, 
   for (int i = 0; i < n; i++) { /* retained trajectory for mplb_get_actions / mplb_get_seg_states (traj_ stays as it was on failure) */
     /* lhm_ is NOT refreshed by plan(): the link table stays whatever getLinkedNodes built last (map_planner.cpp:127) */
     if (results[i].status != MPLB_PLAN_OK) continue;
-    const int ns = std::min(results[i].n_seg, max_seg);
+    const int ns = results[i].n_seg;
     acts.resize(std::max(ns, 1));
     segs.resize((size_t)std::max(ns, 1) * 13);
-    LPA_CUDA(cudaMemcpy(acts.data(), lead->acts.p + (size_t)i * max_seg, (size_t)ns * sizeof(int), cudaMemcpyDeviceToHost));
-    LPA_CUDA(cudaMemcpy(segs.data(), lead->segs.p + (size_t)i * max_seg * 13, (size_t)ns * 13 * sizeof(double), cudaMemcpyDeviceToHost));
+    const int *d_acts = lead->acts.p + (size_t)i * max_seg;
+    const double *d_segs = lead->segs.p + (size_t)i * max_seg * 13;
+    TmpBuf<int> long_acts;
+    TmpBuf<double> long_segs;
+    if (ns > max_seg) { /* the launch kept max_seg rows; traj_act / best on the device still hold the whole trajectory */
+      LPA_CUDA(long_acts.grow(ns, 0));
+      LPA_CUDA(long_segs.grow((size_t)ns * 13, 0));
+      k_lpa_traj<<<(ns + 127) / 128, 128>>>(ctxs.p + i, ns, long_acts.p, long_segs.p);
+      mplb_internal_count_launches(1);
+      LPA_CUDA(cudaGetLastError());
+      d_acts = long_acts.p;
+      d_segs = long_segs.p;
+    }
+    LPA_CUDA(cudaMemcpy(acts.data(), d_acts, (size_t)ns * sizeof(int), cudaMemcpyDeviceToHost));
+    LPA_CUDA(cudaMemcpy(segs.data(), d_segs, (size_t)ns * 13 * sizeof(double), cudaMemcpyDeviceToHost));
     mplb_internal_set_retained(ps[i], &results[i], acts.data(), segs.data(), ns);
   }
   return MPLB_OK;
@@ -657,6 +699,21 @@ int mplb_lpa_get_heap(mplb_planner *p, mplb_lpa_heap_entry *out, int cap) {
   LPA_CUDA(cudaMemcpy(nodes.data(), s->nodes.p, nodes.size() * sizeof(Node), cudaMemcpyDeviceToHost));
   for (int i = 0; i < hd.n_heap && i < cap; i++) { out[i].fval = f[i]; out[i].key_hash = key_hash(nodes[hn[i]].key, s->h.cfg.nkey); }
   return hd.n_heap;
+}
+
+int mplb_lpa_get_capacity(mplb_planner *p, int32_t *cap_nodes, int32_t *cap_pred, int32_t *tsize, int32_t *n_nodes_physical,
+                          int32_t *grows) {
+  Session *s = need(p, "lpa_get_capacity");
+  if (!s) return MPLB_ERR_STATE;
+  Hdr hd;
+  int rc = read_hdr(s, &hd);
+  if (rc) return rc;
+  if (cap_nodes) *cap_nodes = s->cap_nodes;
+  if (cap_pred) *cap_pred = s->cap_pred;
+  if (tsize) *tsize = s->tsize;
+  if (n_nodes_physical) *n_nodes_physical = hd.n_nodes;
+  if (grows) *grows = s->grows;
+  return MPLB_OK;
 }
 
 int mplb_lpa_get_best_child(mplb_planner *p, mplb_lpa_node *out, int cap) {

@@ -319,6 +319,8 @@ class MapPlanner:
     def setMemFraction(self, f): self._set("mem_fraction", f)
     def setMaxSlots(self, n): self._set("max_slots", n)
     def setArenaBytes(self, n): self._set("arena_bytes", n)  # upper bound on the arena budget; 0 = unset
+    def setLPAInitNodes(self, n): self._set("lpa_init_nodes", n)  # LPA* node capacity at allocation (default 65 536)
+    def setLPAInitPreds(self, n): self._set("lpa_init_preds", n)  # LPA* predecessor records at allocation (default 2^20)
 
     def setDt(self, dt):
         self._set("dt", dt)
@@ -487,6 +489,13 @@ class MapPlanner:
         a = np.zeros(max(n, 1), dtype=_lib.LPA_NODE_DTYPE)
         n = check(lib().mplb_lpa_get_best_child(self._h, ptr(a), a.size))
         return a[:n]
+
+    def lpaCapacity(self):
+        """capacity of the LPA* session's device arrays (mplb_lpa_get_capacity): cap_nodes, cap_pred, tsize,
+        n_nodes_physical (records in use, those a getSubStateSpace dropped from hm_ included) and grows (doublings)"""
+        v = [C.c_int32() for _ in range(5)]
+        check(lib().mplb_lpa_get_capacity(self._h, *[C.byref(x) for x in v]))
+        return dict(zip(("cap_nodes", "cap_pred", "tsize", "n_nodes_physical", "grows"), (x.value for x in v)))
 
     def result(self):
         return self._last

@@ -7,6 +7,10 @@
  * for the link table and the voxel matching, growth of the arrays between a stopped and a resumed plan), so that the CPU test
  * suite can compare the core with the checker (oracle) where no GPU exists.  g++ -O2 -ffp-contract=off.  The product has no
  * CPU path: libmplb.so does not contain this file.
+ * Overruns: every array is allocated with GUARD spare elements beyond its capacity, and after every call into the core the
+ * counters are checked against the capacities the core was given (n_nodes, n_order, n_heap <= cap_nodes, n_pred <= cap_pred,
+ * n_links <= cap_links).  A write past a capacity therefore lands in owned memory and is reported (emu_overrun) instead of
+ * being hidden by a vector's spare room or corrupting the heap.
  */
 #include <algorithm>
 #include <cstdio>
@@ -21,6 +25,7 @@
 using namespace mplb_lpa;
 
 namespace {
+constexpr int GUARD = LPA_MAXU + 1; /* spare elements behind every capacity: more than one pop or one plan entry can overrun */
 struct EmuMap {
   int dim;
   int nd[3];
@@ -38,6 +43,8 @@ struct Emu {
   int init_cap = 1 << 16, init_pred = 1 << 20;
   int grows = 0;
   int serial_finish = 0;
+  int no_start_room = 0; /* test switch: skip the host's room-for-the-start-node growth (shows what the invariant check catches) */
+  std::string overrun;   /* first capacity violation seen, empty if none */
   /* "device" arrays */
   Hdr hdr{};
   std::vector<Node> nodes; std::vector<Succ> succ; std::vector<Pred> preds; std::vector<int> table, order, order2, heap_node, best, traj_act, epq_node, link_count;
@@ -60,10 +67,21 @@ struct Emu {
     x.link_count = link_count.data(); x.match = match.data();
     return x;
   }
+  void check(const char *where) { /* the capacities the core was given hold after every call into it */
+    const Hdr &h = hdr;
+    if (!overrun.empty()) return;
+    if (h.n_nodes > cap_nodes || h.n_order > cap_nodes || h.n_heap > cap_nodes || h.n_pred > cap_pred || h.n_links > h.cap_links) {
+      char b[256];
+      std::snprintf(b, sizeof(b), "%s: n_nodes %d n_order %d n_heap %d (cap_nodes %d), n_pred %d (cap_pred %d), n_links %d (cap_links %d)",
+                    where, h.n_nodes, h.n_order, h.n_heap, cap_nodes, h.n_pred, cap_pred, h.n_links, h.cap_links);
+      overrun = b;
+    }
+  }
   void ensure(int cap, int cpred) { /* ensure_capacity of mplb_lpa.cu */
     if (cap > cap_nodes) {
-      nodes.resize(cap); succ.resize((size_t)cap * nU); order.resize(cap); order2.resize(cap); heap_f.resize(cap); heap_node.resize(cap);
-      best.resize(cap); traj_act.resize(cap); mark.resize(cap); link_count.resize(cap);
+      const size_t c = (size_t)cap + GUARD;
+      nodes.resize(c); succ.resize(c * nU); order.resize(c); order2.resize(c); heap_f.resize(c); heap_node.resize(c);
+      best.resize(c); traj_act.resize(c); mark.resize(c); link_count.resize(c);
       cap_nodes = cap;
       int ts = 1024;
       while (ts < 2 * cap) ts <<= 1;
@@ -73,14 +91,14 @@ struct Emu {
       Ctx x = ctx();
       for (int i = 0; i < hdr.n_nodes; i++) table_insert(x, i); /* k_lpa_rehash */
     }
-    if (cpred > cap_pred) { preds.resize(cpred); cap_pred = cpred; }
+    if (cpred > cap_pred) { preds.resize((size_t)cpred + GUARD); cap_pred = cpred; }
     rows.resize(std::max(nU, 32));
     hdr.cap_nodes = cap_nodes; hdr.cap_pred = cap_pred; hdr.tsize = tsize;
   }
   void reset() {
     nodes.clear(); succ.clear(); preds.clear(); table.clear(); order.clear(); order2.clear(); heap_node.clear(); best.clear(); traj_act.clear();
     heap_f.clear(); mark.clear(); link_count.clear(); links.clear(); match.clear();
-    cap_nodes = cap_pred = tsize = 0; have_links = false; control = 0;
+    cap_nodes = cap_pred = tsize = 0; have_links = false; control = 0; grows = 0;
     std::memset(&hdr, 0, sizeof(hdr));
   }
 };
@@ -117,8 +135,9 @@ int emu_planner_set_param(void *pp, const char *key, double v) {
   const std::string k(key);
   if (k == "v_max") p->v_max = v; else if (k == "a_max") p->a_max = v; else if (k == "j_max") p->j_max = v; else if (k == "dt") p->dt = v;
   else if (k == "w") p->w = v; else if (k == "epsilon") p->eps = v; else if (k == "max_num") p->max_num = (int)v; else if (k == "tol_pos") p->tol_pos = v;
-  else if (k == "tol_vel") p->tol_vel = v; else if (k == "tol_acc") p->tol_acc = v; else if (k == "init_cap") p->init_cap = (int)v;
-  else if (k == "init_pred") p->init_pred = (int)v; else if (k == "serial_finish") p->serial_finish = (int)v; else return -1;
+  else if (k == "tol_vel") p->tol_vel = v; else if (k == "tol_acc") p->tol_acc = v; else if (k == "init_cap" || k == "lpa_init_nodes") p->init_cap = (int)v;
+  else if (k == "init_pred" || k == "lpa_init_preds") p->init_pred = (int)v; else if (k == "serial_finish") p->serial_finish = (int)v;
+  else if (k == "no_start_room") p->no_start_room = (int)v; else return -1;
   return 0;
 }
 void emu_planner_set_controls(void *pp, const double *U, int n, int udim) {
@@ -128,12 +147,18 @@ void emu_planner_set_controls(void *pp, const double *U, int n, int udim) {
   p->nU = n;
 }
 int emu_grows(void *pp) { return ((Emu *)pp)->grows; }
+const char *emu_overrun(void *pp) { return ((Emu *)pp)->overrun.c_str(); }
+void emu_capacity(void *pp, int32_t *out5) { /* mplb_lpa_get_capacity */
+  Emu *p = (Emu *)pp;
+  out5[0] = p->cap_nodes; out5[1] = p->cap_pred; out5[2] = p->tsize; out5[3] = p->hdr.n_nodes; out5[4] = p->grows;
+}
 void emu_lpa_reset(void *pp) { ((Emu *)pp)->reset(); }
 
 int emu_lpa_plan(void *pp, const orc_waypoint *start, const orc_waypoint *goal, orc_result *out) {
   Emu *p = (Emu *)pp;
   p->control = start->control;
   if (p->cap_nodes == 0) p->ensure(p->init_cap, p->init_pred);
+  if (!p->no_start_room && p->hdr.n_nodes + 1 > p->cap_nodes) { p->grows++; p->ensure(p->cap_nodes * 2, p->cap_pred * 2); } /* room for the start node */
   p->hdr.resume = 0; p->hdr.status = 0;
   int code;
   while (true) { /* one iteration = one launch of k_lpa_plan */
@@ -143,9 +168,11 @@ int emu_lpa_plan(void *pp, const orc_waypoint *start, const orc_waypoint *goal, 
       double sst[13], gst[13];
       wp_state(*start, sst); wp_state(*goal, gst);
       code = plan_begin(x, sst, start->t, gst);
+      p->check("plan_begin");
     }
     while (code == -1) {
       const int r = pop_begin(x);
+      p->check("pop_begin");
       if (r == -1) {
         const Node &n = x.nodes[x.h->curr];
         for (int lane = 0; lane < 32; lane++) for (int u = lane; u < x.cfg.nU; u += 32) succ_row(x.cfg, n.st, n.t, n.key, u, &x.rows[u]);
@@ -153,6 +180,7 @@ int emu_lpa_plan(void *pp, const orc_waypoint *start, const orc_waypoint *goal, 
       if (r == -1 || r == -2) {
         if (p->serial_finish) code = pop_finish(x);                      /* the one-lane tail */
         else { PopScratch S; pop_finish_warp(x, &S); code = S.ret; }     /* the warp-wide tail, lane loops serialised */
+        p->check("pop_finish");
       } else code = r;
     }
     if (code == LPA_NEED_GROW) { p->hdr.resume = 1; p->grows++; p->ensure(p->cap_nodes * 2, p->cap_pred * 2); continue; }
@@ -164,6 +192,7 @@ int emu_lpa_plan(void *pp, const orc_waypoint *start, const orc_waypoint *goal, 
   int n_seg = 0;
   double cost = LPA_INF;
   if (code == LPA_OK) code = recover(x, &n_seg, &cost); else if (code == LPA_START_IS_GOAL) cost = 0;
+  p->check("recover");
   h.status = code;
   orc_result r;
   std::memset(&r, 0, sizeof(r));
@@ -188,6 +217,7 @@ int emu_lpa_get_sub_state_space(void *pp, int k) {
   if (edges + p->nU > (size_t)p->cap_pred) p->ensure(p->cap_nodes, (int)(edges + p->nU));
   Ctx x = p->ctx();
   const int st = sub_state_space(x, k);
+  p->check("sub_state_space");
   return st == LPA_FAULT ? -1 : p->hdr.n_order;
 }
 int emu_lpa_get_linked_nodes(void *pp, double *pts3, int cap) {
@@ -198,9 +228,11 @@ int emu_lpa_get_linked_nodes(void *pp, double *pts3, int cap) {
   int run = 0;
   for (int i = 0; i < p->hdr.n_order; i++) { const int c = x.link_count[i]; x.link_count[i] = run; run += c; } /* k_lpa_link_scan */
   p->hdr.n_links = run;
-  p->links.resize(run + 1);
+  p->links.resize((size_t)run + GUARD);
+  p->hdr.cap_links = run;
   x = p->ctx();
   for (int i = p->hdr.n_order - 1; i >= 0; i--) link_node(x, i, x.links + x.link_count[i]); /* k_lpa_link_fill, any thread order */
+  p->check("link_node");
   for (int i = 0; i < run && i < cap; i++)
     for (int k = 0; k < 3; k++) pts3[(size_t)i * 3 + k] = k < p->dim ? ((double)p->links[i].cell[k] + 0.5) * x.cfg.res + x.cfg.origin[k] : 0.0;
   return run;
@@ -216,6 +248,7 @@ static int emu_update(Emu *p, const int32_t *c3, int n, bool blocked) {
     }
   std::sort(m.begin(), m.end()); /* k_lpa_apply */
   for (unsigned long long key : m) { const Link &l = p->links[(int)(key % (unsigned long long)p->hdr.n_links)]; apply_change(x, l.node, l.pred_idx, blocked); }
+  p->check(blocked ? "apply_change (blocked)" : "apply_change (cleared)");
   return (int)m.size();
 }
 int emu_lpa_update_blocked_nodes(void *pp, const int32_t *c3, int n) { return emu_update((Emu *)pp, c3, n, true); }

@@ -34,6 +34,9 @@ def lib(reverse=False):
         L.emu_planner_set_param.argtypes = [C.c_void_p, C.c_char_p, C.c_double]
         L.emu_planner_set_controls.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
         L.emu_grows.argtypes = [C.c_void_p]
+        L.emu_overrun.restype = C.c_char_p
+        L.emu_overrun.argtypes = [C.c_void_p]
+        L.emu_capacity.argtypes = [C.c_void_p, C.c_void_p]
         _LIBS[reverse] = L
     return _LIBS[reverse]
 
@@ -58,9 +61,27 @@ class EmuMap:
         map_set_cells(lib(self.REV), "emu_", self.h, cells, value)
 
 
+class EmuOverrun(AssertionError):
+    """the device core wrote past a capacity it was given (found by the host build's invariant check)"""
+
+
+def _checked(name):
+    def call(self, *a):
+        out = getattr(LpaMixin, name)(self, *a)
+        msg = lib(self.REV).emu_overrun(self.h).decode()
+        if msg:
+            raise EmuOverrun(msg)
+        return out
+    return call
+
+
 class EmuPlanner(LpaMixin):
+    """every LPA* call raises EmuOverrun as soon as the core has exceeded one of its capacities"""
     _lpa_prefix = "emu_"
     REV = False
+    for _n in ("lpa_plan", "lpa_get_sub_state_space", "lpa_get_linked_nodes", "lpa_update_blocked_nodes", "lpa_update_cleared_nodes"):
+        locals()[_n] = _checked(_n)
+    del _n
 
     @classmethod
     def _lpa_lib(cls):
@@ -83,6 +104,20 @@ class EmuPlanner(LpaMixin):
 
     def grows(self):
         return lib(self.REV).emu_grows(self.h)
+
+    def lpa_actions(self):
+        f = lib(self.REV).emu_lpa_get_actions
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
+        n = f(self.h, None, 0)
+        a = np.zeros(max(n, 1), dtype=np.int32)
+        n = f(self.h, _ptr(a), a.size)
+        return a[:n]
+
+    def lpa_capacity(self):
+        """the emulator's counterpart of mplb_lpa_get_capacity"""
+        a = np.zeros(5, dtype=np.int32)
+        lib(self.REV).emu_capacity(self.h, _ptr(a))
+        return dict(zip(("cap_nodes", "cap_pred", "tsize", "n_nodes_physical", "grows"), (int(x) for x in a)))
 
 
 class EmuMapRev(EmuMap):

@@ -44,7 +44,7 @@ class GpuPlanner:
         self.pl.setMapUtil(m.mu)
 
     def set_param(self, key, v):
-        if key in ("tol_pos", "tol_vel", "tol_acc", "max_num", "epsilon"):
+        if key in ("tol_pos", "tol_vel", "tol_acc", "max_num", "epsilon", "lpa_init_nodes", "lpa_init_preds"):
             self.pl._set(key, v)
         else:
             {"v_max": self.pl.setVmax, "a_max": self.pl.setAmax, "j_max": self.pl.setJmax, "dt": self.pl.setDt, "w": self.pl.setW}[key](v)
