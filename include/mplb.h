@@ -256,12 +256,33 @@ int mplb_serialize_trajectories(mplb_planner *p, const mplb_result *results, con
  *   n_segs       (may be NULL) segments of trajectory i's result: W_i - 1, or 0 where the reference returns an empty
  *                Trajectory (fewer than two waypoints, solver not initialised)
  * Host buffers; the _device variant takes wps / dts / coefs in HBM (wp_offsets and n_segs stay host arrays) and orders its
- * work on `stream`.  FP64, every operation in the reference's order with Eigen's unblocked partial-pivot LU restated
- * (DESIGN.md section 4.11 states what that pins and the tolerance against a real Eigen build). */
+ * work on `stream`, returning once the solve has completed.  The _device variant also takes a sub-range of a larger list:
+ * wp_offsets[0] may be any value, and offsets are then relative to it — d_wps points at waypoint wp_offsets[0], while d_dts and
+ * d_coefs start at that sub-range's first segment (the host variant requires wp_offsets[0] = 0).  Both variants write every
+ * coefficient slot of the range: the slots of trajectories they do not solve (solver not initialised) are zeroed.
+ * FP64, every operation in the reference's order with Eigen's unblocked partial-pivot LU restated (DESIGN.md section 4.11
+ * states what that pins, the shared-memory / global-scratch split, and the measured accuracy).  A call whose work space in
+ * global scratch would exceed 8 GiB (about 7 800 waypoints for 3-D JRK with a JRK yaw) fails with MPLB_ERR_NOMEM. */
 int mplb_traj_solve_batch(int dim, int control, int yaw_control, int n_traj, const int32_t *wp_offsets, const mplb_waypoint *wps,
                           const double *dts, double *coefs, int32_t *n_segs);
 int mplb_traj_solve_batch_device(int dim, int control, int yaw_control, int n_traj, const int32_t *wp_offsets, const void *d_wps,
                                  const void *d_dts, void *d_coefs, int32_t *n_segs, void *stream);
+
+/* What the last trajectory solve issued by the calling host thread launched (mplb_traj_solve_batch(_device) or
+ * mplb_refine_trajectories(_device)); all zero after a call that launched nothing or failed.  One solve is a pair of CTAs per
+ * trajectory, position axes and yaw, and each CTA keeps its work space in shared memory when it fits smem_bytes and in
+ * global scratch otherwise, so the two CTAs of one trajectory can differ. */
+typedef struct mplb_traj_solve_stats {
+  int32_t n_traj;       /* trajectories solved (CTA pairs launched) */
+  int32_t max_wp;       /* largest waypoint count among them */
+  int32_t pos_shared;   /* position CTAs whose work space was in shared memory */
+  int32_t pos_global;   /* ... in global scratch */
+  int32_t yaw_shared;   /* yaw CTAs in shared memory */
+  int32_t yaw_global;   /* yaw CTAs in global scratch */
+  int64_t smem_bytes;   /* dynamic shared memory per CTA of the launch */
+  int64_t global_bytes; /* global scratch the launch used (0 when every CTA fit in shared memory) */
+} mplb_traj_solve_stats;
+int mplb_traj_solve_last_stats(mplb_traj_solve_stats *out);
 
 /* The refinement step of map_planner_node.cpp:216-227 for a whole batch without leaving the device: for every successful plan of
  * mplb_plan_batch(_device) (same max_seg; results, actions and seg_states are all required) the waypoints of its trajectory

@@ -28,7 +28,10 @@ LPA_HEAP_DTYPE = np.dtype([("fval", "f8"), ("key_hash", "u8")], align=True)
 TIER_DTYPE = np.dtype([("cap", "i4"), ("slots", "i4"), ("n_work", "i4"), ("n_overflow", "i4"), ("hcap", "i4"), ("load_inv", "i4"),
                        ("tsize_max", "i4"), ("log_cap", "i4"), ("stride_bytes", "i8"), ("nomem", "i4"), ("ordered", "i4"),
                        ("resident", "i4"), ("reserved", "i4")], align=True)
+TRAJ_STATS_DTYPE = np.dtype([("n_traj", "i4"), ("max_wp", "i4"), ("pos_shared", "i4"), ("pos_global", "i4"), ("yaw_shared", "i4"),
+                             ("yaw_global", "i4"), ("smem_bytes", "i8"), ("global_bytes", "i8")], align=True)
 assert WAYPOINT_DTYPE.itemsize == 120 and RESULT_DTYPE.itemsize == 80 and TIER_DTYPE.itemsize == 56
+assert TRAJ_STATS_DTYPE.itemsize == 40
 
 # every symbol include/mplb.h declares: (restype, argtypes)
 _VP, _I, _D = C.c_void_p, C.c_int, C.c_double
@@ -98,6 +101,7 @@ SYMBOLS = {
     "mplb_refine_trajectories": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _I, _VP, _VP]),
     "mplb_traj_solve_batch": (_I, [_I, _I, _I, _I, _VP, _VP, _VP, _VP, _VP]),
     "mplb_traj_solve_batch_device": (_I, [_I, _I, _I, _I, _VP, _VP, _VP, _VP, _VP, _VP]),
+    "mplb_traj_solve_last_stats": (_I, [_VP]),
     "mplb_trajectory_msg_size": (C.c_size_t, [_I, C.c_char_p]),
     "mplb_serialize_trajectories_device": (_I, [_VP, _VP, _VP, _VP, _I, _I, _D, C.c_uint32, C.c_uint32, C.c_uint32, C.c_char_p,
                                                 _VP, C.c_size_t, _VP, _VP]),

@@ -361,6 +361,7 @@ struct TsScratch { /* grow-only staging buffer on the device that was current wh
   }
 };
 thread_local TsScratch g_jobs, g_ws, g_wps, g_dts, g_coefs;
+thread_local mplb_traj_solve_stats g_stats; /* what the last ts_run of this host thread launched */
 
 #define TS_CUDA(expr)                                                                                         \
   do {                                                                                                        \
@@ -371,6 +372,7 @@ thread_local TsScratch g_jobs, g_ws, g_wps, g_dts, g_coefs;
 /* launches the solve for `jobs` (wp_off / n_wp / seg_off filled by the caller; ws_off is assigned here) */
 int ts_run(int dim, int Np, int Rp, int Ny, int Ry, int yaw_control, std::vector<TsJob> &jobs, const mplb_waypoint *d_wps,
            const double *d_dts, double *d_coefs, cudaStream_t stream) {
+  g_stats = mplb_traj_solve_stats{};
   size_t ws_total = 0, ws_max = 0;
   for (TsJob &j : jobs) {
     j.ws_off = (long long)ws_total;
@@ -384,14 +386,22 @@ int ts_run(int dim, int Np, int Rp, int Ny, int Ry, int yaw_control, std::vector
   TS_CUDA(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
   const size_t smem_cap = (size_t)std::max(0, smem_optin - 1024);
   const size_t smem_bytes = std::min(ws_max * sizeof(double), smem_cap) / 8 * 8;
-  bool need_global = false;
-  for (const TsJob &j : jobs)
-    if (std::max(ts_ws_doubles(j.n_wp, Np, dim), ts_ws_doubles(j.n_wp, Ny, 1)) * sizeof(double) > smem_bytes) need_global = true;
+  mplb_traj_solve_stats st{};
+  st.n_traj = (int32_t)jobs.size();
+  st.smem_bytes = (int64_t)smem_bytes;
+  for (const TsJob &j : jobs) { /* the kernel's per-CTA test: need <= smem_bytes / 8 */
+    const bool pos_g = ts_ws_doubles(j.n_wp, Np, dim) > smem_bytes / 8, yaw_g = ts_ws_doubles(j.n_wp, Ny, 1) > smem_bytes / 8;
+    (pos_g ? st.pos_global : st.pos_shared)++;
+    (yaw_g ? st.yaw_global : st.yaw_shared)++;
+    st.max_wp = std::max(st.max_wp, (int32_t)j.n_wp);
+  }
+  const bool need_global = st.pos_global + st.yaw_global > 0;
   TS_CUDA(g_jobs.reserve(jobs.size() * sizeof(TsJob)));
   if (need_global) {
     /* the dense formulation is O(W^2) memory per trajectory like the reference's (segments*N)^2 matrices: refuse absurd sizes */
     if (ws_total * sizeof(double) > ((size_t)8 << 30)) return mplb_internal_fail(MPLB_ERR_NOMEM, "traj_solve: work space above 8 GiB (waypoint lists this long are out of this solver's range)");
     TS_CUDA(g_ws.reserve(ws_total * sizeof(double)));
+    st.global_bytes = (int64_t)(ws_total * sizeof(double));
   }
   TS_CUDA(cudaMemcpyAsync(g_jobs.p, jobs.data(), jobs.size() * sizeof(TsJob), cudaMemcpyHostToDevice, stream));
   TS_CUDA(cudaFuncSetAttribute(k_traj_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
@@ -400,6 +410,7 @@ int ts_run(int dim, int Np, int Rp, int Ny, int Ry, int yaw_control, std::vector
   mplb_internal_count_launches(1);
   TS_CUDA(cudaGetLastError());
   TS_CUDA(cudaStreamSynchronize(stream)); /* the job list is reused by the next call */
+  g_stats = st;
   return MPLB_OK;
 }
 
@@ -409,7 +420,7 @@ int ts_launch(int dim, int control, int yaw_control, int n_traj, const int32_t *
   const bool ok = ts_orders(control, &Np, &Rp) && (yaw_control == 1 || yaw_control == 3 || yaw_control == 7) &&
                   ts_orders(yaw_control, &Ny, &Ry);
   std::vector<TsJob> jobs;
-  int seg_off = 0;
+  int seg_off = 0, unsolved_slots = 0;
   for (int i = 0; i < n_traj; i++) {
     const int W = wp_offsets[i + 1] - wp_offsets[i];
     const int slots = std::max(W - 1, 0);
@@ -417,10 +428,16 @@ int ts_launch(int dim, int control, int yaw_control, int n_traj, const int32_t *
     if (n_segs) n_segs[i] = nseg;
     const int my_off = seg_off;
     seg_off += slots;
+    unsolved_slots += slots - nseg;
     if (!nseg) continue;
     TsJob j;
     j.wp_off = wp_offsets[i] - wp_offsets[0]; j.n_wp = W; j.seg_off = my_off; j.pad = 0; j.ws_off = 0;
     jobs.push_back(j);
+  }
+  if (unsolved_slots) { /* only an uninitialised solver leaves slots unsolved, and then it leaves all of them: zero them like
+                          the host variant does, and return once that is done as a solve would */
+    TS_CUDA(cudaMemsetAsync(d_coefs, 0, (size_t)seg_off * (dim + 1) * 6 * sizeof(double), stream));
+    if (jobs.empty()) TS_CUDA(cudaStreamSynchronize(stream));
   }
   return ts_run(dim, Np, Rp, Ny, Ry, yaw_control, jobs, d_wps, d_dts, d_coefs, stream);
 }
@@ -468,6 +485,12 @@ thread_local TsScratch g_pwps, g_pdts, g_pU, g_pres;
 }  // namespace
 
 extern "C" {
+
+int mplb_traj_solve_last_stats(mplb_traj_solve_stats *out) {
+  if (!out) return mplb_internal_fail(MPLB_ERR_ARG, "traj_solve_last_stats: null output");
+  *out = g_stats;
+  return MPLB_OK;
+}
 
 int mplb_traj_solve_batch_device(int dim, int control, int yaw_control, int n_traj, const int32_t *wp_offsets,
                                  const void *d_wps, const void *d_dts, void *d_coefs, int32_t *n_segs, void *stream) {

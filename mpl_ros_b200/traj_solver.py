@@ -40,6 +40,14 @@ def solve_batch(dim, control, waypoint_lists, dts_lists, yaw_control=VEL):
     return out
 
 
+def last_stats():
+    """What the last solve of this thread launched (mplb_traj_solve_last_stats): dict of n_traj, max_wp, pos_shared, pos_global,
+    yaw_shared, yaw_global, smem_bytes and global_bytes."""
+    st = np.zeros(1, dtype=_lib.TRAJ_STATS_DTYPE)
+    check(lib().mplb_traj_solve_last_stats(ptr(st)))
+    return {k: int(st[0][k]) for k in _lib.TRAJ_STATS_DTYPE.names}
+
+
 class TrajSolver:
     """traj_solver.h:12-109."""
 

@@ -30,6 +30,16 @@ def test_struct_layouts_match_header():
     assert oracle.WAYPOINT_DTYPE == _lib.WAYPOINT_DTYPE and oracle.RESULT_DTYPE == _lib.RESULT_DTYPE
 
 
+def test_traj_solve_stats_layout():
+    """mplb_traj_solve_stats: six int32 counters, then two int64 byte counts (include/mplb.h)."""
+    from mpl_ros_b200 import _lib
+    d = _lib.TRAJ_STATS_DTYPE
+    assert d.itemsize == 40 and d.fields["smem_bytes"][1] == 24 and d.fields["global_bytes"][1] == 32
+    hdr = open(os.path.join(ROOT, "include", "mplb.h")).read()
+    body = hdr[hdr.index("typedef struct mplb_traj_solve_stats"):hdr.index("} mplb_traj_solve_stats;")]
+    assert re.findall(r"int(?:32|64)_t (\w+);", body) == list(d.names)
+
+
 def test_no_device_is_a_loud_error():
     """Without a CUDA device the planner must fail, not fall back."""
     import pytest

@@ -12,6 +12,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 TESTS = ["tests/test_oracle_vs_reference.py", "tests/test_oracle_fuzz_vs_reference.py", "tests/test_gpu_vs_reference.py",
          "tests/test_oracle_trajsolver.py::test_oracle_equals_reference_sources",
+         "tests/test_oracle_trajsolver_edges.py::test_oracle_equals_reference_sources",
          "tests/test_oracle_lpa.py::test_oracle_equals_reference_sources"]
 
 
