@@ -1,7 +1,13 @@
 /* mplb_internal.h — host helpers the translation units of libmplb.so share (not part of the ABI). */
 #ifndef MPLB_INTERNAL_H
 #define MPLB_INTERNAL_H
+#include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <algorithm>
+#include <string>
+
+#include "../../include/mplb.h"
 #if defined(__GNUC__)
 #define MPLB_HIDDEN __attribute__((visibility("hidden")))
 #else
@@ -11,6 +17,61 @@
 MPLB_HIDDEN int mplb_internal_fail(int code, const char *msg);
 /* adds to the counter behind mplb_launch_count() */
 MPLB_HIDDEN void mplb_internal_count_launches(int n);
+/* makes `device` the calling thread's current device; 0 on success, -1 when it cannot be selected */
+MPLB_HIDDEN int mplb_internal_set_device(int device);
+
+/* returns MPLB_ERR_CUDA from the enclosing function when `expr` (a cudaError_t) is not cudaSuccess */
+#define MPLB_CUDA_TRY(expr)                                                                                              \
+  do {                                                                                                                   \
+    cudaError_t e__ = (expr);                                                                                            \
+    if (e__ != cudaSuccess)                                                                                              \
+      return mplb_internal_fail(MPLB_ERR_CUDA, (std::string(#expr) + ": " + cudaGetErrorString(e__)).c_str());         \
+  } while (0)
+
+/* An owned device array of n elements of T, freed when the buffer is destroyed (the result of that cudaFree is ignored: at
+ * process exit it may be cudaErrorCudartUnloading).  Movable, not copyable. */
+template <class T>
+struct MPLB_HIDDEN DevBuf {
+  T *p = nullptr;
+  size_t n = 0;
+
+  DevBuf() = default;
+  DevBuf(const DevBuf &) = delete;
+  DevBuf &operator=(const DevBuf &) = delete;
+  DevBuf(DevBuf &&o) noexcept : p(o.p), n(o.n) { o.p = nullptr; o.n = 0; }
+  DevBuf &operator=(DevBuf &&o) noexcept {
+    if (this != &o) { release(); p = o.p; n = o.n; o.p = nullptr; o.n = 0; }
+    return *this;
+  }
+  ~DevBuf() { release(); }
+
+  void release() {
+    if (p) cudaFree(p);
+    p = nullptr;
+    n = 0;
+  }
+  /* at least `want` elements, contents discarded: the old array is freed before the new one is allocated */
+  cudaError_t reserve(size_t want) {
+    if (want <= n) return cudaSuccess;
+    release();
+    T *q = nullptr;
+    cudaError_t e = cudaMalloc((void **)&q, want * sizeof(T));
+    if (e == cudaSuccess) { p = q; n = want; }
+    return e;
+  }
+  /* at least `want` elements keeping the first `keep`: the new array is allocated and filled before the old one is freed */
+  cudaError_t grow(size_t want, size_t keep) {
+    if (want <= n) return cudaSuccess;
+    T *q = nullptr;
+    cudaError_t e = cudaMalloc((void **)&q, want * sizeof(T));
+    if (e != cudaSuccess) return e;
+    if (p && keep) e = cudaMemcpy(q, p, std::min(keep, n) * sizeof(T), cudaMemcpyDeviceToDevice);
+    release();
+    p = q;
+    n = want;
+    return e;
+  }
+};
 
 /* ---- what the LPA* unit (mplb_lpa.cu) needs from the planner / map objects of mplb.cu */
 struct mplb_planner;

@@ -39,12 +39,6 @@ using namespace mplb_lpa;
 
 namespace {
 
-#define LPA_CUDA(expr)                                                                                          \
-  do {                                                                                                          \
-    cudaError_t e__ = (expr);                                                                                   \
-    if (e__ != cudaSuccess) return mplb_internal_fail(MPLB_ERR_CUDA, (std::string(#expr) + ": " + cudaGetErrorString(e__)).c_str()); \
-  } while (0)
-
 __device__ void wp_to_state(const mplb_waypoint &w, double *st) {
   for (int k = 0; k < 3; k++) { st[k] = w.pos[k]; st[3 + k] = w.vel[k]; st[6 + k] = w.acc[k]; st[9 + k] = w.jrk[k]; }
   st[12] = w.yaw;
@@ -219,54 +213,29 @@ __global__ void k_lpa_traj(const Ctx *ctx, int n_seg, int *acts, double *segs) {
 }
 
 /* ------------------------------------------------------------------ host side */
-template <typename T>
-struct Buf {
-  T *p = nullptr;
-  size_t n = 0;
-  cudaError_t grow(size_t want, size_t keep) { /* reallocate to `want` elements, keeping the first `keep` */
-    if (want <= n) return cudaSuccess;
-    T *q = nullptr;
-    cudaError_t e = cudaMalloc((void **)&q, want * sizeof(T));
-    if (e != cudaSuccess) return e;
-    if (p && keep) e = cudaMemcpy(q, p, std::min(keep, n) * sizeof(T), cudaMemcpyDeviceToDevice);
-    if (p) cudaFree(p);
-    p = q; n = want;
-    return e;
-  }
-  void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
-};
-template <typename T>
-struct TmpBuf : Buf<T> { ~TmpBuf() { this->release(); } }; /* freed on every return path */
-
 struct Session {
   bool on = false;
   int device = 0;
   int control = 0; /* Control flags of the first start waypoint: fixes the lattice key layout */
   Ctx h{};         /* host copy (device pointers inside) */
-  Buf<Ctx> d_ctx;
-  Buf<Hdr> d_hdr;
-  Buf<Node> nodes;
-  Buf<Succ> succ;
-  Buf<Pred> preds;
-  Buf<int> table, order, order2, heap_node, best, traj_act, epq_node, link_count, cells;
-  Buf<double> heap_f, epq_f, U, segs;
-  Buf<Row> rows;
-  Buf<unsigned char> mark;
-  Buf<Link> links;
-  Buf<unsigned long long> match;
-  Buf<mplb_waypoint> wps;
-  Buf<mplb_result> res;
-  Buf<int> acts;
+  DevBuf<Ctx> d_ctx;
+  DevBuf<Hdr> d_hdr;
+  DevBuf<Node> nodes;
+  DevBuf<Succ> succ;
+  DevBuf<Pred> preds;
+  DevBuf<int> table, order, order2, heap_node, best, traj_act, epq_node, link_count, cells;
+  DevBuf<double> heap_f, epq_f, U, segs;
+  DevBuf<Row> rows;
+  DevBuf<unsigned char> mark;
+  DevBuf<Link> links;
+  DevBuf<unsigned long long> match;
+  DevBuf<mplb_waypoint> wps;
+  DevBuf<mplb_result> res;
+  DevBuf<int> acts;
   int cap_nodes = 0, cap_pred = 0, tsize = 0, nU = 0, n_links_host = 0;
   int init_nodes = 1 << 16, init_pred = 1 << 20; /* MPLB_LPA_INIT_NODES / _PREDS, read at every plan, used when allocating */
   int grows = 0;                                 /* doublings since the arrays were allocated */
   bool have_links = false;
-  void release() {
-    d_ctx.release(); d_hdr.release(); nodes.release(); succ.release(); preds.release(); table.release(); order.release();
-    order2.release(); heap_node.release(); best.release(); traj_act.release(); epq_node.release(); link_count.release();
-    cells.release(); heap_f.release(); epq_f.release(); U.release(); segs.release(); rows.release(); mark.release();
-    links.release(); match.release(); wps.release(); res.release(); acts.release();
-  }
 };
 
 std::unordered_map<mplb_planner *, Session *> g_sessions; /* planner -> its replanning session; the registry is locked, a
@@ -284,12 +253,12 @@ Session *session_of(mplb_planner *p, bool create) {
 }
 
 int upload_ctx(Session *s) {
-  LPA_CUDA(s->d_ctx.grow(1, 0));
-  LPA_CUDA(cudaMemcpy(s->d_ctx.p, &s->h, sizeof(Ctx), cudaMemcpyHostToDevice));
+  MPLB_CUDA_TRY(s->d_ctx.grow(1, 0));
+  MPLB_CUDA_TRY(cudaMemcpy(s->d_ctx.p, &s->h, sizeof(Ctx), cudaMemcpyHostToDevice));
   return MPLB_OK;
 }
-int read_hdr(Session *s, Hdr *out) { LPA_CUDA(cudaMemcpy(out, s->d_hdr.p, sizeof(Hdr), cudaMemcpyDeviceToHost)); return MPLB_OK; }
-int write_hdr(Session *s, const Hdr &in) { LPA_CUDA(cudaMemcpy(s->d_hdr.p, &in, sizeof(Hdr), cudaMemcpyHostToDevice)); return MPLB_OK; }
+int read_hdr(Session *s, Hdr *out) { MPLB_CUDA_TRY(cudaMemcpy(out, s->d_hdr.p, sizeof(Hdr), cudaMemcpyDeviceToHost)); return MPLB_OK; }
+int write_hdr(Session *s, const Hdr &in) { MPLB_CUDA_TRY(cudaMemcpy(s->d_hdr.p, &in, sizeof(Hdr), cudaMemcpyHostToDevice)); return MPLB_OK; }
 
 /* (re)size the node-indexed arrays to `cap` nodes and the predecessor pool to `cap_pred`; contents survive */
 int ensure_capacity(Session *s, int cap, int cap_pred, bool keep) {
@@ -299,32 +268,32 @@ int ensure_capacity(Session *s, int cap, int cap_pred, bool keep) {
   const size_t used = keep ? (size_t)hd.n_nodes : 0;
   const bool grow_nodes = cap > s->cap_nodes;
   if (grow_nodes) {
-    LPA_CUDA(s->nodes.grow(cap, used));
-    LPA_CUDA(s->succ.grow((size_t)cap * s->nU, used * s->nU));
-    LPA_CUDA(s->order.grow(cap, keep ? (size_t)hd.n_order : 0));
-    LPA_CUDA(s->order2.grow(cap, 0));
-    LPA_CUDA(s->heap_f.grow(cap, keep ? (size_t)hd.n_heap : 0));
-    LPA_CUDA(s->heap_node.grow(cap, keep ? (size_t)hd.n_heap : 0));
-    LPA_CUDA(s->best.grow(cap, keep ? (size_t)hd.n_best : 0));
-    LPA_CUDA(s->traj_act.grow(cap, 0));
-    LPA_CUDA(s->mark.grow(cap, 0));
-    LPA_CUDA(s->link_count.grow(cap, 0));
+    MPLB_CUDA_TRY(s->nodes.grow(cap, used));
+    MPLB_CUDA_TRY(s->succ.grow((size_t)cap * s->nU, used * s->nU));
+    MPLB_CUDA_TRY(s->order.grow(cap, keep ? (size_t)hd.n_order : 0));
+    MPLB_CUDA_TRY(s->order2.grow(cap, 0));
+    MPLB_CUDA_TRY(s->heap_f.grow(cap, keep ? (size_t)hd.n_heap : 0));
+    MPLB_CUDA_TRY(s->heap_node.grow(cap, keep ? (size_t)hd.n_heap : 0));
+    MPLB_CUDA_TRY(s->best.grow(cap, keep ? (size_t)hd.n_best : 0));
+    MPLB_CUDA_TRY(s->traj_act.grow(cap, 0));
+    MPLB_CUDA_TRY(s->mark.grow(cap, 0));
+    MPLB_CUDA_TRY(s->link_count.grow(cap, 0));
     s->cap_nodes = cap;
     int ts = 1024;
     while (ts < 2 * cap) ts <<= 1;
     if (ts > s->tsize) {
       s->table.release();
-      LPA_CUDA(s->table.grow(ts, 0));
+      MPLB_CUDA_TRY(s->table.grow(ts, 0));
       s->tsize = ts;
     }
-    LPA_CUDA(cudaMemset(s->table.p, 0xff, (size_t)s->tsize * sizeof(int)));
+    MPLB_CUDA_TRY(cudaMemset(s->table.p, 0xff, (size_t)s->tsize * sizeof(int)));
   }
   if (cap_pred > s->cap_pred) {
-    LPA_CUDA(s->preds.grow(cap_pred, keep ? (size_t)hd.n_pred : 0));
+    MPLB_CUDA_TRY(s->preds.grow(cap_pred, keep ? (size_t)hd.n_pred : 0));
     s->cap_pred = cap_pred;
   }
-  LPA_CUDA(s->d_hdr.grow(1, 1));
-  LPA_CUDA(s->rows.grow(std::max(s->nU, 32), 0)); /* >= one staging row per lane (re-created successors of a stored list) */
+  MPLB_CUDA_TRY(s->d_hdr.grow(1, 1));
+  MPLB_CUDA_TRY(s->rows.grow(std::max(s->nU, 32), 0)); /* >= one staging row per lane (re-created successors of a stored list) */
   s->h.h = s->d_hdr.p; s->h.nodes = s->nodes.p; s->h.succ = s->succ.p; s->h.preds = s->preds.p; s->h.table = s->table.p;
   s->h.order = s->order.p; s->h.order2 = s->order2.p; s->h.heap_f = s->heap_f.p; s->h.heap_node = s->heap_node.p;
   s->h.best = s->best.p; s->h.traj_act = s->traj_act.p; s->h.rows = s->rows.p; s->h.mark = s->mark.p;
@@ -337,8 +306,8 @@ int ensure_capacity(Session *s, int cap, int cap_pred, bool keep) {
   if (grow_nodes && keep && hd.n_nodes > 0) {
     k_lpa_rehash<<<1, 32>>>(s->d_ctx.p);
     mplb_internal_count_launches(1);
-    LPA_CUDA(cudaGetLastError());
-    LPA_CUDA(cudaDeviceSynchronize());
+    MPLB_CUDA_TRY(cudaGetLastError());
+    MPLB_CUDA_TRY(cudaDeviceSynchronize());
   }
   return MPLB_OK;
 }
@@ -357,12 +326,12 @@ int refresh_cfg(mplb_planner *p, Session *s, int control) {
   if (!ord) return mplb_internal_fail(MPLB_ERR_ARG, "LPA*: the start waypoint carries no control flag");
   if (s->control && s->control != control) return mplb_internal_fail(MPLB_ERR_ARG, "LPA*: the control flag changed since the first plan; call mplb_planner_reset first");
   if (s->nU && s->nU != hc.nU) return mplb_internal_fail(MPLB_ERR_ARG, "LPA*: the control set changed since the first plan; call mplb_planner_reset first");
-  LPA_CUDA(cudaSetDevice(hc.device));
+  MPLB_CUDA_TRY(cudaSetDevice(hc.device));
   s->device = hc.device;
   s->nU = hc.nU;
   s->init_nodes = hc.lpa_init_nodes; s->init_pred = hc.lpa_init_preds;
-  LPA_CUDA(s->U.grow((size_t)hc.nU * 3, 0));
-  LPA_CUDA(cudaMemcpy(s->U.p, hc.U, (size_t)hc.nU * 3 * sizeof(double), cudaMemcpyHostToDevice));
+  MPLB_CUDA_TRY(s->U.grow((size_t)hc.nU * 3, 0));
+  MPLB_CUDA_TRY(cudaMemcpy(s->U.p, hc.U, (size_t)hc.nU * 3 * sizeof(double), cudaMemcpyHostToDevice));
   Cfg &c = s->h.cfg;
   c.dim = hc.dim; c.ord = ord; c.control = control; c.nU = hc.nU; c.nkey = hc.dim * ord; c.max_num = hc.max_num;
   c.dt = hc.dt; c.w = hc.w; c.eps = hc.eps; c.v_max = hc.v_max; c.a_max = hc.a_max; c.j_max = hc.j_max;
@@ -373,11 +342,9 @@ int refresh_cfg(mplb_planner *p, Session *s, int control) {
 }
 
 int reset_state(Session *s) { /* PlannerBase::reset: the next plan starts a new StateSpace (and may use other controls) */
-  s->release();
-  s->cap_nodes = 0; s->cap_pred = 0; s->tsize = 0; s->nU = 0; s->n_links_host = 0; s->grows = 0;
-  s->have_links = false;
-  s->control = 0;
-  std::memset(&s->h, 0, sizeof(s->h));
+  Session fresh; /* frees every array when it replaces *s; only the switch, the device and the initial sizes stay */
+  fresh.on = s->on; fresh.device = s->device; fresh.init_nodes = s->init_nodes; fresh.init_pred = s->init_pred;
+  *s = std::move(fresh);
   return MPLB_OK;
 }
 
@@ -410,23 +377,22 @@ int plan_sessions(std::vector<mplb_planner *> &ps, const mplb_waypoint *starts, 
   /* the batch's contexts, contiguous */
   Session *lead = ss[0];
   const int max_seg = 4096; /* per-plan trajectory rows of the launch; longer trajectories are gathered after it */
-  TmpBuf<Ctx> ctxs;
-  LPA_CUDA(ctxs.grow(n, 0));
-  for (int i = 0; i < n; i++) LPA_CUDA(cudaMemcpy(ctxs.p + i, &ss[i]->h, sizeof(Ctx), cudaMemcpyHostToDevice));
-  LPA_CUDA(lead->wps.grow((size_t)2 * n, 0));
-  LPA_CUDA(lead->res.grow(n, 0));
-  LPA_CUDA(lead->acts.grow((size_t)n * max_seg, 0));
-  LPA_CUDA(lead->segs.grow((size_t)n * max_seg * 13, 0));
-  LPA_CUDA(cudaMemcpy(lead->wps.p, starts, (size_t)n * sizeof(mplb_waypoint), cudaMemcpyHostToDevice));
-  LPA_CUDA(cudaMemcpy(lead->wps.p + n, goals, (size_t)n * sizeof(mplb_waypoint), cudaMemcpyHostToDevice));
+  DevBuf<Ctx> ctxs;
+  MPLB_CUDA_TRY(ctxs.grow(n, 0));
+  for (int i = 0; i < n; i++) MPLB_CUDA_TRY(cudaMemcpy(ctxs.p + i, &ss[i]->h, sizeof(Ctx), cudaMemcpyHostToDevice));
+  MPLB_CUDA_TRY(lead->wps.grow((size_t)2 * n, 0));
+  MPLB_CUDA_TRY(lead->res.grow(n, 0));
+  MPLB_CUDA_TRY(lead->acts.grow((size_t)n * max_seg, 0));
+  MPLB_CUDA_TRY(lead->segs.grow((size_t)n * max_seg * 13, 0));
+  MPLB_CUDA_TRY(cudaMemcpy(lead->wps.p, starts, (size_t)n * sizeof(mplb_waypoint), cudaMemcpyHostToDevice));
+  MPLB_CUDA_TRY(cudaMemcpy(lead->wps.p + n, goals, (size_t)n * sizeof(mplb_waypoint), cudaMemcpyHostToDevice));
   for (int i = 0; i < n; i++) { Hdr hd; int rc = read_hdr(ss[i], &hd); if (rc) return rc; hd.resume = 0; hd.status = 0; rc = write_hdr(ss[i], hd); if (rc) return rc; }
   /* every round doubles the arrays of the sessions that stopped, so 64 rounds cannot run out before int capacities do */
   for (int round = 0; round < 64; round++) {
     k_lpa_plan<<<n, 32>>>(ctxs.p, lead->wps.p, lead->wps.p + n, lead->res.p, lead->acts.p, lead->segs.p, max_seg);
     mplb_internal_count_launches(1);
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) return mplb_internal_fail(MPLB_ERR_CUDA, (std::string("k_lpa_plan: ") + cudaGetErrorString(e)).c_str());
+    MPLB_CUDA_TRY(cudaGetLastError());
+    MPLB_CUDA_TRY(cudaDeviceSynchronize());
     bool again = false;
     for (int i = 0; i < n; i++) {
       Hdr hd;
@@ -435,13 +401,13 @@ int plan_sessions(std::vector<mplb_planner *> &ps, const mplb_waypoint *starts, 
       if (hd.status == LPA_NEED_GROW) { /* stopped before a pop that could overflow: double and resume */
         rc = grow_session(ss[i]);
         if (rc) return rc;
-        LPA_CUDA(cudaMemcpy(ctxs.p + i, &ss[i]->h, sizeof(Ctx), cudaMemcpyHostToDevice));
+        MPLB_CUDA_TRY(cudaMemcpy(ctxs.p + i, &ss[i]->h, sizeof(Ctx), cudaMemcpyHostToDevice));
         again = true;
       }
     }
     if (!again) break;
   }
-  LPA_CUDA(cudaMemcpy(results, lead->res.p, (size_t)n * sizeof(mplb_result), cudaMemcpyDeviceToHost));
+  MPLB_CUDA_TRY(cudaMemcpy(results, lead->res.p, (size_t)n * sizeof(mplb_result), cudaMemcpyDeviceToHost));
   std::vector<int> acts;
   std::vector<double> segs;
   for (int i = 0; i < n; i++) { /* retained trajectory for mplb_get_actions / mplb_get_seg_states (traj_ stays as it was on failure) */
@@ -452,19 +418,19 @@ int plan_sessions(std::vector<mplb_planner *> &ps, const mplb_waypoint *starts, 
     segs.resize((size_t)std::max(ns, 1) * 13);
     const int *d_acts = lead->acts.p + (size_t)i * max_seg;
     const double *d_segs = lead->segs.p + (size_t)i * max_seg * 13;
-    TmpBuf<int> long_acts;
-    TmpBuf<double> long_segs;
+    DevBuf<int> long_acts;
+    DevBuf<double> long_segs;
     if (ns > max_seg) { /* the launch kept max_seg rows; traj_act / best on the device still hold the whole trajectory */
-      LPA_CUDA(long_acts.grow(ns, 0));
-      LPA_CUDA(long_segs.grow((size_t)ns * 13, 0));
+      MPLB_CUDA_TRY(long_acts.grow(ns, 0));
+      MPLB_CUDA_TRY(long_segs.grow((size_t)ns * 13, 0));
       k_lpa_traj<<<(ns + 127) / 128, 128>>>(ctxs.p + i, ns, long_acts.p, long_segs.p);
       mplb_internal_count_launches(1);
-      LPA_CUDA(cudaGetLastError());
+      MPLB_CUDA_TRY(cudaGetLastError());
       d_acts = long_acts.p;
       d_segs = long_segs.p;
     }
-    LPA_CUDA(cudaMemcpy(acts.data(), d_acts, (size_t)ns * sizeof(int), cudaMemcpyDeviceToHost));
-    LPA_CUDA(cudaMemcpy(segs.data(), d_segs, (size_t)ns * 13 * sizeof(double), cudaMemcpyDeviceToHost));
+    MPLB_CUDA_TRY(cudaMemcpy(acts.data(), d_acts, (size_t)ns * sizeof(int), cudaMemcpyDeviceToHost));
+    MPLB_CUDA_TRY(cudaMemcpy(segs.data(), d_segs, (size_t)ns * 13 * sizeof(double), cudaMemcpyDeviceToHost));
     mplb_internal_set_retained(ps[i], &results[i], acts.data(), segs.data(), ns);
   }
   return MPLB_OK;
@@ -487,12 +453,12 @@ int build_links(Session *s) {
   k_lpa_link_count<<<blocks, 128>>>(s->d_ctx.p);
   k_lpa_link_scan<<<1, 1>>>(s->d_ctx.p);
   mplb_internal_count_launches(2);
-  LPA_CUDA(cudaGetLastError());
-  LPA_CUDA(cudaDeviceSynchronize());
+  MPLB_CUDA_TRY(cudaGetLastError());
+  MPLB_CUDA_TRY(cudaDeviceSynchronize());
   rc = read_hdr(s, &hd);
   if (rc) return rc;
   if ((size_t)hd.n_links > s->links.n) {
-    LPA_CUDA(s->links.grow((size_t)hd.n_links + 1024, 0));
+    MPLB_CUDA_TRY(s->links.grow((size_t)hd.n_links + 1024, 0));
     s->h.links = s->links.p;
     hd.cap_links = (int)s->links.n;
     rc = write_hdr(s, hd);
@@ -503,8 +469,8 @@ int build_links(Session *s) {
   if (hd.n_links > 0) {
     k_lpa_link_fill<<<blocks, 128>>>(s->d_ctx.p);
     mplb_internal_count_launches(1);
-    LPA_CUDA(cudaGetLastError());
-    LPA_CUDA(cudaDeviceSynchronize());
+    MPLB_CUDA_TRY(cudaGetLastError());
+    MPLB_CUDA_TRY(cudaDeviceSynchronize());
   }
   s->n_links_host = hd.n_links;
   return MPLB_OK;
@@ -517,8 +483,8 @@ int update_nodes(mplb_planner *p, const int32_t *cells3, int n, bool blocked) {
   if (!s->have_links || n == 0 || s->n_links_host == 0) return 0; /* lhm_ empty: nothing is linked (map_planner.cpp:164-168) */
   int rc = refresh_cfg(p, s, s->control); /* the map pointer may have been rebuilt */
   if (rc) return rc;
-  LPA_CUDA(s->cells.grow((size_t)n * 3, 0));
-  LPA_CUDA(cudaMemcpy(s->cells.p, cells3, (size_t)n * 3 * sizeof(int), cudaMemcpyHostToDevice));
+  MPLB_CUDA_TRY(s->cells.grow((size_t)n * 3, 0));
+  MPLB_CUDA_TRY(cudaMemcpy(s->cells.p, cells3, (size_t)n * 3 * sizeof(int), cudaMemcpyHostToDevice));
   Hdr hd;
   for (int attempt = 0; attempt < 2; attempt++) {
     rc = read_hdr(s, &hd);
@@ -531,19 +497,19 @@ int update_nodes(mplb_planner *p, const int32_t *cells3, int n, bool blocked) {
     if (rc) return rc;
     k_lpa_match<<<(s->n_links_host + 127) / 128, 128>>>(s->d_ctx.p, s->cells.p, n);
     mplb_internal_count_launches(1);
-    LPA_CUDA(cudaGetLastError());
-    LPA_CUDA(cudaDeviceSynchronize());
+    MPLB_CUDA_TRY(cudaGetLastError());
+    MPLB_CUDA_TRY(cudaDeviceSynchronize());
     rc = read_hdr(s, &hd);
     if (rc) return rc;
     if ((size_t)hd.n_match <= s->match.n) break;
-    LPA_CUDA(s->match.grow((size_t)hd.n_match + 1024, 0)); /* the pair list did not fit: size it and match again */
+    MPLB_CUDA_TRY(s->match.grow((size_t)hd.n_match + 1024, 0)); /* the pair list did not fit: size it and match again */
     s->h.match = s->match.p;
   }
   if (hd.n_match > 0) {
     k_lpa_apply<<<1, 32>>>(s->d_ctx.p, blocked ? 1 : 0);
     mplb_internal_count_launches(1);
-    LPA_CUDA(cudaGetLastError());
-    LPA_CUDA(cudaDeviceSynchronize());
+    MPLB_CUDA_TRY(cudaGetLastError());
+    MPLB_CUDA_TRY(cudaDeviceSynchronize());
   }
   return hd.n_match;
 }
@@ -562,7 +528,6 @@ void mplb_internal_lpa_drop(mplb_planner *p) {
   std::lock_guard<std::mutex> lock(g_sessions_mu);
   auto it = g_sessions.find(p);
   if (it == g_sessions.end()) return;
-  it->second->release();
   delete it->second;
   g_sessions.erase(it);
 }
@@ -604,16 +569,16 @@ int mplb_get_sub_state_space(mplb_planner *p, int time_step) {
   if (time_step < 0 || time_step >= hd.n_best) return mplb_internal_fail(MPLB_ERR_ARG, "getSubStateSpace: time_step beyond the last trajectory");
   /* scratch of the sweep: one queue entry per stored edge at most, one predecessor record per stored edge at most */
   const size_t edges = (size_t)hd.n_nodes * s->nU + 16;
-  LPA_CUDA(s->epq_f.grow(edges, 0));
-  LPA_CUDA(s->epq_node.grow(edges, 0));
+  MPLB_CUDA_TRY(s->epq_f.grow(edges, 0));
+  MPLB_CUDA_TRY(s->epq_node.grow(edges, 0));
   s->h.epq_f = s->epq_f.p; s->h.epq_node = s->epq_node.p;
   if (edges + (size_t)s->nU > (size_t)s->cap_pred) { rc = ensure_capacity(s, s->cap_nodes, (int)std::min<size_t>(edges + s->nU, 0x7fffffff), true); if (rc) return rc; }
   rc = upload_ctx(s);
   if (rc) return rc;
   k_lpa_subtree<<<1, 32>>>(s->d_ctx.p, time_step);
   mplb_internal_count_launches(1);
-  LPA_CUDA(cudaGetLastError());
-  LPA_CUDA(cudaDeviceSynchronize());
+  MPLB_CUDA_TRY(cudaGetLastError());
+  MPLB_CUDA_TRY(cudaDeviceSynchronize());
   rc = read_hdr(s, &hd);
   if (rc) return rc;
   if (hd.status == LPA_FAULT) return mplb_internal_fail(MPLB_ERR_STATE, "getSubStateSpace: a stored successor is no longer in the state space (the reference dereferences a null State here, state_space.h:160-163)");
@@ -632,7 +597,7 @@ int mplb_get_linked_nodes(mplb_planner *p, double *pts3, int cap) {
   const int n = s->n_links_host;
   if (pts3 && cap > 0 && n > 0) {
     std::vector<Link> l(n);
-    LPA_CUDA(cudaMemcpy(l.data(), s->links.p, (size_t)n * sizeof(Link), cudaMemcpyDeviceToHost));
+    MPLB_CUDA_TRY(cudaMemcpy(l.data(), s->links.p, (size_t)n * sizeof(Link), cudaMemcpyDeviceToHost));
     const Cfg &c = s->h.cfg;
     for (int i = 0; i < n && i < cap; i++) /* intToFloat (map_util.h:110-114): (pn + 0.5) * res + origin */
       for (int k = 0; k < 3; k++) pts3[(size_t)i * 3 + k] = k < c.dim ? ((double)l[i].cell[k] + 0.5) * c.res + c.origin[k] : 0.0;
@@ -656,10 +621,10 @@ int mplb_lpa_get_nodes(mplb_planner *p, mplb_lpa_node *out, int cap) {
   std::vector<Succ> succ((size_t)hd.n_nodes * s->nU);
   std::vector<Pred> preds(std::max(hd.n_pred, 1));
   std::vector<int> order(hd.n_order);
-  LPA_CUDA(cudaMemcpy(nodes.data(), s->nodes.p, nodes.size() * sizeof(Node), cudaMemcpyDeviceToHost));
-  LPA_CUDA(cudaMemcpy(succ.data(), s->succ.p, succ.size() * sizeof(Succ), cudaMemcpyDeviceToHost));
-  if (hd.n_pred > 0) LPA_CUDA(cudaMemcpy(preds.data(), s->preds.p, (size_t)hd.n_pred * sizeof(Pred), cudaMemcpyDeviceToHost));
-  LPA_CUDA(cudaMemcpy(order.data(), s->order.p, order.size() * sizeof(int), cudaMemcpyDeviceToHost));
+  MPLB_CUDA_TRY(cudaMemcpy(nodes.data(), s->nodes.p, nodes.size() * sizeof(Node), cudaMemcpyDeviceToHost));
+  MPLB_CUDA_TRY(cudaMemcpy(succ.data(), s->succ.p, succ.size() * sizeof(Succ), cudaMemcpyDeviceToHost));
+  if (hd.n_pred > 0) MPLB_CUDA_TRY(cudaMemcpy(preds.data(), s->preds.p, (size_t)hd.n_pred * sizeof(Pred), cudaMemcpyDeviceToHost));
+  MPLB_CUDA_TRY(cudaMemcpy(order.data(), s->order.p, order.size() * sizeof(int), cudaMemcpyDeviceToHost));
   const int nk = s->h.cfg.nkey;
   for (int i = 0; i < hd.n_order && i < cap; i++) {
     const Node &n = nodes[order[i]];
@@ -694,9 +659,9 @@ int mplb_lpa_get_heap(mplb_planner *p, mplb_lpa_heap_entry *out, int cap) {
   std::vector<double> f(hd.n_heap);
   std::vector<int> hn(hd.n_heap);
   std::vector<Node> nodes(hd.n_nodes);
-  LPA_CUDA(cudaMemcpy(f.data(), s->heap_f.p, f.size() * sizeof(double), cudaMemcpyDeviceToHost));
-  LPA_CUDA(cudaMemcpy(hn.data(), s->heap_node.p, hn.size() * sizeof(int), cudaMemcpyDeviceToHost));
-  LPA_CUDA(cudaMemcpy(nodes.data(), s->nodes.p, nodes.size() * sizeof(Node), cudaMemcpyDeviceToHost));
+  MPLB_CUDA_TRY(cudaMemcpy(f.data(), s->heap_f.p, f.size() * sizeof(double), cudaMemcpyDeviceToHost));
+  MPLB_CUDA_TRY(cudaMemcpy(hn.data(), s->heap_node.p, hn.size() * sizeof(int), cudaMemcpyDeviceToHost));
+  MPLB_CUDA_TRY(cudaMemcpy(nodes.data(), s->nodes.p, nodes.size() * sizeof(Node), cudaMemcpyDeviceToHost));
   for (int i = 0; i < hd.n_heap && i < cap; i++) { out[i].fval = f[i]; out[i].key_hash = key_hash(nodes[hn[i]].key, s->h.cfg.nkey); }
   return hd.n_heap;
 }
@@ -724,11 +689,11 @@ int mplb_lpa_get_best_child(mplb_planner *p, mplb_lpa_node *out, int cap) {
   if (rc) return rc;
   if (!out || cap <= 0 || hd.n_best == 0) return hd.n_best;
   std::vector<int> best(hd.n_best);
-  LPA_CUDA(cudaMemcpy(best.data(), s->best.p, best.size() * sizeof(int), cudaMemcpyDeviceToHost));
+  MPLB_CUDA_TRY(cudaMemcpy(best.data(), s->best.p, best.size() * sizeof(int), cudaMemcpyDeviceToHost));
   const int nk = s->h.cfg.nkey;
   for (int i = 0; i < hd.n_best && i < cap; i++) {
     Node n;
-    LPA_CUDA(cudaMemcpy(&n, s->nodes.p + best[i], sizeof(Node), cudaMemcpyDeviceToHost));
+    MPLB_CUDA_TRY(cudaMemcpy(&n, s->nodes.p + best[i], sizeof(Node), cudaMemcpyDeviceToHost));
     mplb_lpa_node &o = out[i];
     std::memset(&o, 0, sizeof(o));
     for (int k = 0; k < nk; k++) o.key[k] = n.key[k];

@@ -344,30 +344,20 @@ bool ts_orders(int control, int *N, int *R) { /* traj_solver.h:21-27 */
   return false;
 }
 
-struct TsScratch { /* grow-only staging buffer on the device that was current when it was last grown */
-  void *p = nullptr;
-  size_t bytes = 0;
+/* staging bytes of one host thread on the device that was current when they were last grown (a different current device
+ * reallocates them there); freed when the thread exits */
+struct TsScratch : DevBuf<char> {
   int dev = -1;
   cudaError_t reserve(size_t want) {
     int cur = 0;
     cudaError_t e = cudaGetDevice(&cur);
     if (e != cudaSuccess) return e;
-    if (cur == dev && want <= bytes) return cudaSuccess;
-    if (p) cudaFree(p);
-    p = nullptr; bytes = 0; dev = cur;
-    e = cudaMalloc(&p, want);
-    if (e == cudaSuccess) bytes = want;
-    return e;
+    if (cur != dev) { release(); dev = cur; }
+    return DevBuf<char>::reserve(want);
   }
 };
 thread_local TsScratch g_jobs, g_ws, g_wps, g_dts, g_coefs;
 thread_local mplb_traj_solve_stats g_stats; /* what the last ts_run of this host thread launched */
-
-#define TS_CUDA(expr)                                                                                         \
-  do {                                                                                                        \
-    cudaError_t e__ = (expr);                                                                                 \
-    if (e__ != cudaSuccess) return mplb_internal_fail(MPLB_ERR_CUDA, (std::string(#expr) + ": " + cudaGetErrorString(e__)).c_str()); \
-  } while (0)
 
 /* launches the solve for `jobs` (wp_off / n_wp / seg_off filled by the caller; ws_off is assigned here) */
 int ts_run(int dim, int Np, int Rp, int Ny, int Ry, int yaw_control, std::vector<TsJob> &jobs, const mplb_waypoint *d_wps,
@@ -382,8 +372,8 @@ int ts_run(int dim, int Np, int Rp, int Ny, int Ry, int yaw_control, std::vector
   }
   if (jobs.empty()) return MPLB_OK;
   int dev = 0, smem_optin = 0;
-  TS_CUDA(cudaGetDevice(&dev));
-  TS_CUDA(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  MPLB_CUDA_TRY(cudaGetDevice(&dev));
+  MPLB_CUDA_TRY(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
   const size_t smem_cap = (size_t)std::max(0, smem_optin - 1024);
   const size_t smem_bytes = std::min(ws_max * sizeof(double), smem_cap) / 8 * 8;
   mplb_traj_solve_stats st{};
@@ -396,20 +386,20 @@ int ts_run(int dim, int Np, int Rp, int Ny, int Ry, int yaw_control, std::vector
     st.max_wp = std::max(st.max_wp, (int32_t)j.n_wp);
   }
   const bool need_global = st.pos_global + st.yaw_global > 0;
-  TS_CUDA(g_jobs.reserve(jobs.size() * sizeof(TsJob)));
+  MPLB_CUDA_TRY(g_jobs.reserve(jobs.size() * sizeof(TsJob)));
   if (need_global) {
     /* the dense formulation is O(W^2) memory per trajectory like the reference's (segments*N)^2 matrices: refuse absurd sizes */
     if (ws_total * sizeof(double) > ((size_t)8 << 30)) return mplb_internal_fail(MPLB_ERR_NOMEM, "traj_solve: work space above 8 GiB (waypoint lists this long are out of this solver's range)");
-    TS_CUDA(g_ws.reserve(ws_total * sizeof(double)));
+    MPLB_CUDA_TRY(g_ws.reserve(ws_total * sizeof(double)));
     st.global_bytes = (int64_t)(ws_total * sizeof(double));
   }
-  TS_CUDA(cudaMemcpyAsync(g_jobs.p, jobs.data(), jobs.size() * sizeof(TsJob), cudaMemcpyHostToDevice, stream));
-  TS_CUDA(cudaFuncSetAttribute(k_traj_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+  MPLB_CUDA_TRY(cudaMemcpyAsync(g_jobs.p, jobs.data(), jobs.size() * sizeof(TsJob), cudaMemcpyHostToDevice, stream));
+  MPLB_CUDA_TRY(cudaFuncSetAttribute(k_traj_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
   k_traj_solve<<<dim3((unsigned)jobs.size(), 2), TS_THREADS, smem_bytes, stream>>>(
       (const TsJob *)g_jobs.p, d_wps, d_dts, d_coefs, dim, Np, Rp, Ny, Ry, yaw_control, (double *)g_ws.p, (int)(smem_bytes / 8));
   mplb_internal_count_launches(1);
-  TS_CUDA(cudaGetLastError());
-  TS_CUDA(cudaStreamSynchronize(stream)); /* the job list is reused by the next call */
+  MPLB_CUDA_TRY(cudaGetLastError());
+  MPLB_CUDA_TRY(cudaStreamSynchronize(stream)); /* the job list is reused by the next call */
   g_stats = st;
   return MPLB_OK;
 }
@@ -436,8 +426,8 @@ int ts_launch(int dim, int control, int yaw_control, int n_traj, const int32_t *
   }
   if (unsolved_slots) { /* only an uninitialised solver leaves slots unsolved, and then it leaves all of them: zero them like
                           the host variant does, and return once that is done as a solve would */
-    TS_CUDA(cudaMemsetAsync(d_coefs, 0, (size_t)seg_off * (dim + 1) * 6 * sizeof(double), stream));
-    if (jobs.empty()) TS_CUDA(cudaStreamSynchronize(stream));
+    MPLB_CUDA_TRY(cudaMemsetAsync(d_coefs, 0, (size_t)seg_off * (dim + 1) * 6 * sizeof(double), stream));
+    if (jobs.empty()) MPLB_CUDA_TRY(cudaStreamSynchronize(stream));
   }
   return ts_run(dim, Np, Rp, Ny, Ry, yaw_control, jobs, d_wps, d_dts, d_coefs, stream);
 }
@@ -512,12 +502,12 @@ int mplb_refine_trajectories_device(mplb_planner *p, const void *d_results, cons
   MplbLpaHostCfg hc;
   mplb_internal_planner_cfg(p, &hc);
   if (hc.nU <= 0) return mplb_internal_fail(MPLB_ERR_STATE, "refine: no controls set");
-  TS_CUDA(cudaSetDevice(hc.device));
+  MPLB_CUDA_TRY(cudaSetDevice(hc.device));
   int Np = 0, Rp = 0, Ny = 0, Ry = 0;
   const bool ok = ts_orders(control, &Np, &Rp) && (yaw_control == 1 || yaw_control == 3 || yaw_control == 7) && ts_orders(yaw_control, &Ny, &Ry);
   std::vector<mplb_result> res(n);
-  TS_CUDA(cudaMemcpyAsync(res.data(), d_results, (size_t)n * sizeof(mplb_result), cudaMemcpyDeviceToHost, stream));
-  TS_CUDA(cudaStreamSynchronize(stream));
+  MPLB_CUDA_TRY(cudaMemcpyAsync(res.data(), d_results, (size_t)n * sizeof(mplb_result), cudaMemcpyDeviceToHost, stream));
+  MPLB_CUDA_TRY(cudaStreamSynchronize(stream));
   const int per = max_seg + 1;
   std::vector<TsJob> jobs;
   for (int i = 0; i < n; i++) {
@@ -528,23 +518,23 @@ int mplb_refine_trajectories_device(mplb_planner *p, const void *d_results, cons
     j.wp_off = i * per; j.n_wp = res[i].n_seg + 1; j.seg_off = i * max_seg; j.pad = 0; j.ws_off = 0;
     jobs.push_back(j);
   }
-  TS_CUDA(g_pwps.reserve((size_t)n * per * sizeof(mplb_waypoint)));
-  TS_CUDA(g_pdts.reserve((size_t)n * max_seg * sizeof(double)));
-  TS_CUDA(g_pU.reserve((size_t)hc.nU * 4 * sizeof(double)));
-  TS_CUDA(cudaMemcpyAsync(g_pU.p, hc.U, (size_t)hc.nU * 3 * sizeof(double), cudaMemcpyHostToDevice, stream));
+  MPLB_CUDA_TRY(g_pwps.reserve((size_t)n * per * sizeof(mplb_waypoint)));
+  MPLB_CUDA_TRY(g_pdts.reserve((size_t)n * max_seg * sizeof(double)));
+  MPLB_CUDA_TRY(g_pU.reserve((size_t)hc.nU * 4 * sizeof(double)));
+  MPLB_CUDA_TRY(cudaMemcpyAsync(g_pU.p, hc.U, (size_t)hc.nU * 3 * sizeof(double), cudaMemcpyHostToDevice, stream));
   double *d_Uyaw = nullptr;
   if (hc.Uyaw) {
     d_Uyaw = (double *)g_pU.p + (size_t)hc.nU * 3;
-    TS_CUDA(cudaMemcpyAsync(d_Uyaw, hc.Uyaw, (size_t)hc.nU * sizeof(double), cudaMemcpyHostToDevice, stream));
+    MPLB_CUDA_TRY(cudaMemcpyAsync(d_Uyaw, hc.Uyaw, (size_t)hc.nU * sizeof(double), cudaMemcpyHostToDevice, stream));
   }
-  TS_CUDA(cudaMemsetAsync(d_coefs, 0, (size_t)n * max_seg * (hc.dim + 1) * 6 * sizeof(double), stream));
+  MPLB_CUDA_TRY(cudaMemsetAsync(d_coefs, 0, (size_t)n * max_seg * (hc.dim + 1) * 6 * sizeof(double), stream));
   const long long total = (long long)n * per;
   k_gather_waypoints<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>((const mplb_result *)d_results, (const int *)d_actions,
                                                                            (const double *)d_seg_states, n, max_seg, hc.dim, plan_control,
                                                                            (const double *)g_pU.p, d_Uyaw, hc.dt, (mplb_waypoint *)g_pwps.p,
                                                                            (double *)g_pdts.p);
   mplb_internal_count_launches(1);
-  TS_CUDA(cudaGetLastError());
+  MPLB_CUDA_TRY(cudaGetLastError());
   return ts_run(hc.dim, Np, Rp, Ny, Ry, yaw_control, jobs, (const mplb_waypoint *)g_pwps.p, (const double *)g_pdts.p, (double *)d_coefs, stream);
 }
 
@@ -554,18 +544,18 @@ int mplb_refine_trajectories(mplb_planner *p, const mplb_result *results, const 
   if (n == 0) return MPLB_OK;
   MplbLpaHostCfg hc;
   mplb_internal_planner_cfg(p, &hc);
-  TS_CUDA(cudaSetDevice(hc.device));
+  MPLB_CUDA_TRY(cudaSetDevice(hc.device));
   const size_t nc = (size_t)n * max_seg * (hc.dim + 1) * 6;
-  TS_CUDA(g_pres.reserve((size_t)n * sizeof(mplb_result)));
-  TS_CUDA(g_wps.reserve((size_t)n * max_seg * sizeof(int)));         /* staging: actions */
-  TS_CUDA(g_dts.reserve((size_t)n * max_seg * 13 * sizeof(double))); /* staging: segment states */
-  TS_CUDA(g_coefs.reserve(nc * sizeof(double)));
-  TS_CUDA(cudaMemcpy(g_pres.p, results, (size_t)n * sizeof(mplb_result), cudaMemcpyHostToDevice));
-  TS_CUDA(cudaMemcpy(g_wps.p, actions, (size_t)n * max_seg * sizeof(int), cudaMemcpyHostToDevice));
-  TS_CUDA(cudaMemcpy(g_dts.p, seg_states, (size_t)n * max_seg * 13 * sizeof(double), cudaMemcpyHostToDevice));
+  MPLB_CUDA_TRY(g_pres.reserve((size_t)n * sizeof(mplb_result)));
+  MPLB_CUDA_TRY(g_wps.reserve((size_t)n * max_seg * sizeof(int)));         /* staging: actions */
+  MPLB_CUDA_TRY(g_dts.reserve((size_t)n * max_seg * 13 * sizeof(double))); /* staging: segment states */
+  MPLB_CUDA_TRY(g_coefs.reserve(nc * sizeof(double)));
+  MPLB_CUDA_TRY(cudaMemcpy(g_pres.p, results, (size_t)n * sizeof(mplb_result), cudaMemcpyHostToDevice));
+  MPLB_CUDA_TRY(cudaMemcpy(g_wps.p, actions, (size_t)n * max_seg * sizeof(int), cudaMemcpyHostToDevice));
+  MPLB_CUDA_TRY(cudaMemcpy(g_dts.p, seg_states, (size_t)n * max_seg * 13 * sizeof(double), cudaMemcpyHostToDevice));
   const int rc = mplb_refine_trajectories_device(p, g_pres.p, g_wps.p, g_dts.p, n, max_seg, plan_control, control, yaw_control, g_coefs.p, n_segs, nullptr);
   if (rc != MPLB_OK) return rc;
-  TS_CUDA(cudaMemcpy(coefs, g_coefs.p, nc * sizeof(double), cudaMemcpyDeviceToHost));
+  MPLB_CUDA_TRY(cudaMemcpy(coefs, g_coefs.p, nc * sizeof(double), cudaMemcpyDeviceToHost));
   return MPLB_OK;
 }
 
@@ -583,15 +573,15 @@ int mplb_traj_solve_batch(int dim, int control, int yaw_control, int n_traj, con
     n_seg_total += std::max(wp_offsets[i + 1] - wp_offsets[i] - 1, 0);
   }
   const size_t n_seg_slots = (size_t)std::max(n_seg_total, 1);
-  TS_CUDA(g_wps.reserve((size_t)std::max(n_wp, 1) * sizeof(mplb_waypoint)));
-  TS_CUDA(g_dts.reserve(n_seg_slots * sizeof(double)));
-  TS_CUDA(g_coefs.reserve(n_seg_slots * (dim + 1) * 6 * sizeof(double)));
-  TS_CUDA(cudaMemcpy(g_wps.p, wps, (size_t)n_wp * sizeof(mplb_waypoint), cudaMemcpyHostToDevice));
-  TS_CUDA(cudaMemcpy(g_dts.p, dts, (size_t)n_seg_total * sizeof(double), cudaMemcpyHostToDevice));
-  TS_CUDA(cudaMemset(g_coefs.p, 0, n_seg_slots * (dim + 1) * 6 * sizeof(double)));
+  MPLB_CUDA_TRY(g_wps.reserve((size_t)std::max(n_wp, 1) * sizeof(mplb_waypoint)));
+  MPLB_CUDA_TRY(g_dts.reserve(n_seg_slots * sizeof(double)));
+  MPLB_CUDA_TRY(g_coefs.reserve(n_seg_slots * (dim + 1) * 6 * sizeof(double)));
+  MPLB_CUDA_TRY(cudaMemcpy(g_wps.p, wps, (size_t)n_wp * sizeof(mplb_waypoint), cudaMemcpyHostToDevice));
+  MPLB_CUDA_TRY(cudaMemcpy(g_dts.p, dts, (size_t)n_seg_total * sizeof(double), cudaMemcpyHostToDevice));
+  MPLB_CUDA_TRY(cudaMemset(g_coefs.p, 0, n_seg_slots * (dim + 1) * 6 * sizeof(double)));
   const int rc = mplb_traj_solve_batch_device(dim, control, yaw_control, n_traj, wp_offsets, g_wps.p, g_dts.p, g_coefs.p, n_segs, nullptr);
   if (rc != MPLB_OK) return rc;
-  TS_CUDA(cudaMemcpy(coefs, g_coefs.p, (size_t)n_seg_total * (dim + 1) * 6 * sizeof(double), cudaMemcpyDeviceToHost));
+  MPLB_CUDA_TRY(cudaMemcpy(coefs, g_coefs.p, (size_t)n_seg_total * (dim + 1) * 6 * sizeof(double), cudaMemcpyDeviceToHost));
   return MPLB_OK;
 }
 }

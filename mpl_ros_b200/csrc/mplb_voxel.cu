@@ -36,37 +36,6 @@ using namespace mplb_ref;
 
 namespace {
 
-#define VG_CUDA(expr)                                                                                                   \
-  do {                                                                                                                  \
-    cudaError_t e__ = (expr);                                                                                           \
-    if (e__ != cudaSuccess)                                                                                             \
-      return mplb_internal_fail(MPLB_ERR_CUDA, (std::string(#expr) + ": " + cudaGetErrorString(e__)).c_str());        \
-  } while (0)
-
-int vg_fail(int code, const char *msg) { return mplb_internal_fail(code, msg); }
-
-int set_device(int device) {
-  int cur = -1;
-  if (cudaGetDevice(&cur) != cudaSuccess) return -1;
-  if (cur != device && cudaSetDevice(device) != cudaSuccess) return -1;
-  return 0;
-}
-
-template <typename T>
-struct Buf { /* grow-only device buffer */
-  T *p = nullptr;
-  size_t n = 0;
-  cudaError_t reserve(size_t want) {
-    if (want <= n) return cudaSuccess;
-    if (p) cudaFree(p);
-    p = nullptr; n = 0;
-    cudaError_t e = cudaMalloc((void **)&p, want * sizeof(T));
-    if (e == cudaSuccess) n = want;
-    return e;
-  }
-  void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
-};
-
 /* geometry as the kernels see it */
 struct Geo {
   int nd[3];
@@ -247,27 +216,20 @@ struct mplb_voxel_grid {
   float res = 0;
   size_t ncell = 0;
   int device = 0;
-  int8_t *d_map = nullptr, *d_inf = nullptr;
+  DevBuf<int8_t> d_map, d_inf;
   long long chunk_points = 0;
   /* scratch of the inflated insertion and of the clouds */
-  Buf<unsigned> k0, k1, v0, v1, pcell;
-  Buf<int> flag, pos, ns, cells, rows, obs;
-  Buf<double> pts;
-  Buf<char> tmp;
-  Buf<int8_t> bytes;
+  DevBuf<unsigned> k0, k1, v0, v1, pcell;
+  DevBuf<int> flag, pos, ns, cells, rows, obs;
+  DevBuf<double> pts;
+  DevBuf<char> tmp;
+  DevBuf<int8_t> bytes;
 
   Geo geo() const {
     Geo g;
     for (int i = 0; i < 3; i++) { g.nd[i] = dim[i]; g.origin_d[i] = origin_d[i]; }
     g.res = res;
     return g;
-  }
-  void release() {
-    if (d_map) cudaFree(d_map);
-    if (d_inf) cudaFree(d_inf);
-    d_map = d_inf = nullptr;
-    k0.release(); k1.release(); v0.release(); v1.release(); pcell.release(); flag.release(); pos.release(); ns.release();
-    obs.release(); cells.release(); rows.release(); pts.release(); tmp.release(); bytes.release();
   }
 };
 
@@ -277,8 +239,8 @@ int vg_allocate(mplb_voxel_grid *g, const double *dim_m, const double *origin, i
   int nd[3], no[3];
   for (int i = 0; i < 3; i++) { /* Vec3i new_dim(new_dim_d(i) / res_, ...), the float res_ widened (vg:130-131) */
     const double qd = dim_m[i] / (double)g->res, qo = origin[i] / (double)g->res;
-    if (!(qd > -1.0 && qd < 2147483648.0)) return vg_fail(MPLB_ERR_ARG, "voxel grid dimension negative, NaN or beyond int32");
-    if (!(qo > -2147483649.0 && qo < 2147483648.0)) return vg_fail(MPLB_ERR_ARG, "voxel grid origin NaN or beyond int32");
+    if (!(qd > -1.0 && qd < 2147483648.0)) return mplb_internal_fail(MPLB_ERR_ARG, "voxel grid dimension negative, NaN or beyond int32");
+    if (!(qo > -2147483649.0 && qo < 2147483648.0)) return mplb_internal_fail(MPLB_ERR_ARG, "voxel grid origin NaN or beyond int32");
     nd[i] = (int)qd;
     no[i] = (int)qo;
   }
@@ -288,23 +250,19 @@ int vg_allocate(mplb_voxel_grid *g, const double *dim_m, const double *origin, i
       no[2] == g->ori[2])
     return MPLB_OK; /* vg:134-137 */
   const size_t ncell = (size_t)nd[0] * nd[1] * nd[2];
-  if (ncell > 0x7fffffffull) return vg_fail(MPLB_ERR_ARG, "voxel grid of more than 2^31 - 1 cells");
-  int8_t *m = nullptr, *f = nullptr;
+  if (ncell > 0x7fffffffull) return mplb_internal_fail(MPLB_ERR_ARG, "voxel grid of more than 2^31 - 1 cells");
+  DevBuf<int8_t> m, f;
   if (ncell) {
-    VG_CUDA(cudaMalloc((void **)&m, ncell));
-    cudaError_t e = cudaMalloc((void **)&f, ncell);
-    if (e != cudaSuccess) { cudaFree(m); return vg_fail(MPLB_ERR_CUDA, "cudaMalloc(voxel grid)"); }
-    k_vg_shift<<<blocks_for(ncell), 256>>>(g->d_map, g->dim[0], g->dim[1], g->dim[2], m, nd[0], nd[1], nd[2], no[0] - g->ori[0],
+    MPLB_CUDA_TRY(m.reserve(ncell));
+    MPLB_CUDA_TRY(f.reserve(ncell));
+    k_vg_shift<<<blocks_for(ncell), 256>>>(g->d_map.p, g->dim[0], g->dim[1], g->dim[2], m.p, nd[0], nd[1], nd[2], no[0] - g->ori[0],
                                             no[1] - g->ori[1], no[2] - g->ori[2]);
     mplb_internal_count_launches(1);
-    e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpy(f, m, ncell, cudaMemcpyDeviceToDevice); /* inflated_map_ = new_map (vg:163-164) */
-    if (e != cudaSuccess) { cudaFree(m); cudaFree(f); return vg_fail(MPLB_ERR_CUDA, cudaGetErrorString(e)); }
+    MPLB_CUDA_TRY(cudaGetLastError());
+    MPLB_CUDA_TRY(cudaMemcpy(f.p, m.p, ncell, cudaMemcpyDeviceToDevice)); /* inflated_map_ = new_map (vg:163-164) */
   }
-  if (g->d_map) cudaFree(g->d_map);
-  if (g->d_inf) cudaFree(g->d_inf);
-  g->d_map = m;
-  g->d_inf = f;
+  g->d_map = std::move(m); /* frees the old grids */
+  g->d_inf = std::move(f);
   g->ncell = ncell;
   for (int i = 0; i < 3; i++) { g->dim[i] = nd[i]; g->ori[i] = no[i]; g->origin_d[i] = origin[i]; }
   if (changed) *changed = 1;
@@ -315,9 +273,9 @@ int vg_allocate(mplb_voxel_grid *g, const double *dim_m, const double *origin, i
 template <class F>
 int with_tmp(mplb_voxel_grid *g, F f) {
   size_t bytes = 0;
-  VG_CUDA(f((void *)nullptr, bytes));
-  VG_CUDA(g->tmp.reserve(std::max<size_t>(bytes, 1)));
-  VG_CUDA(f((void *)g->tmp.p, bytes));
+  MPLB_CUDA_TRY(f((void *)nullptr, bytes));
+  MPLB_CUDA_TRY(g->tmp.reserve(std::max<size_t>(bytes, 1)));
+  MPLB_CUDA_TRY(f((void *)g->tmp.p, bytes));
   return MPLB_OK;
 }
 
@@ -326,10 +284,10 @@ long long vg_add_inflated(mplb_voxel_grid *g, const void *d_pts, long long n, in
                           long long cap, cudaStream_t s) {
   if (n <= 0 || n_ns <= 0 || g->ncell == 0) {
     if (n > 0 && g->ncell) { /* no offsets: only map_ changes */
-      k_vg_add<<<blocks_for((size_t)n), 256, 0, s>>>(g->geo(), d_pts, fp32, n, g->d_map);
+      k_vg_add<<<blocks_for((size_t)n), 256, 0, s>>>(g->geo(), d_pts, fp32, n, g->d_map.p);
       mplb_internal_count_launches(1);
-      VG_CUDA(cudaGetLastError());
-      VG_CUDA(cudaStreamSynchronize(s));
+      MPLB_CUDA_TRY(cudaGetLastError());
+      MPLB_CUDA_TRY(cudaStreamSynchronize(s));
     }
     return 0;
   }
@@ -339,44 +297,44 @@ long long vg_add_inflated(mplb_voxel_grid *g, const void *d_pts, long long n, in
   const long long cand = chunk * n_ns;
   const unsigned ncell = (unsigned)g->ncell;
   const int bits = key_bits(ncell);
-  VG_CUDA(g->ns.reserve((size_t)n_ns * 3));
-  VG_CUDA(cudaMemcpyAsync(g->ns.p, h_ns, (size_t)n_ns * 3 * sizeof(int), cudaMemcpyHostToDevice, s));
-  VG_CUDA(g->k0.reserve((size_t)cand)); VG_CUDA(g->k1.reserve((size_t)cand));
-  VG_CUDA(g->v0.reserve((size_t)cand)); VG_CUDA(g->v1.reserve((size_t)cand));
-  VG_CUDA(g->pcell.reserve((size_t)chunk));
-  VG_CUDA(g->flag.reserve((size_t)cand)); VG_CUDA(g->pos.reserve((size_t)cand));
+  MPLB_CUDA_TRY(g->ns.reserve((size_t)n_ns * 3));
+  MPLB_CUDA_TRY(cudaMemcpyAsync(g->ns.p, h_ns, (size_t)n_ns * 3 * sizeof(int), cudaMemcpyHostToDevice, s));
+  MPLB_CUDA_TRY(g->k0.reserve((size_t)cand)); MPLB_CUDA_TRY(g->k1.reserve((size_t)cand));
+  MPLB_CUDA_TRY(g->v0.reserve((size_t)cand)); MPLB_CUDA_TRY(g->v1.reserve((size_t)cand));
+  MPLB_CUDA_TRY(g->pcell.reserve((size_t)chunk));
+  MPLB_CUDA_TRY(g->flag.reserve((size_t)cand)); MPLB_CUDA_TRY(g->pos.reserve((size_t)cand));
   const Geo geo = g->geo();
   long long total = 0;
   for (long long i0 = 0; i0 < n; i0 += chunk) {
     const int np = (int)std::min(chunk, n - i0);
     const long long nc = (long long)np * n_ns;
     k_vg_point_keys<<<blocks_for(np), 256, 0, s>>>(geo, d_pts, fp32, i0, np, ncell, g->k0.p, g->v0.p);
-    VG_CUDA(cudaGetLastError());
+    MPLB_CUDA_TRY(cudaGetLastError());
     int rc = with_tmp(g, [&](void *t, size_t &b) {
       return cub::DeviceRadixSort::SortPairs(t, b, g->k0.p, g->k1.p, g->v0.p, g->v1.p, np, 0, bits, s);
     });
     if (rc) return rc;
-    k_vg_point_first<<<blocks_for(np), 256, 0, s>>>(g->k1.p, g->v1.p, np, ncell, g->d_map, g->pcell.p);
-    k_vg_cand_keys<<<blocks_for(nc), 256, 0, s>>>(g->pcell.p, np, g->ns.p, n_ns, g->dim[0], g->dim[1], g->dim[2], ncell, g->d_inf,
+    k_vg_point_first<<<blocks_for(np), 256, 0, s>>>(g->k1.p, g->v1.p, np, ncell, g->d_map.p, g->pcell.p);
+    k_vg_cand_keys<<<blocks_for(nc), 256, 0, s>>>(g->pcell.p, np, g->ns.p, n_ns, g->dim[0], g->dim[1], g->dim[2], ncell, g->d_inf.p,
                                                   g->k0.p, g->v0.p);
-    VG_CUDA(cudaGetLastError());
+    MPLB_CUDA_TRY(cudaGetLastError());
     rc = with_tmp(g, [&](void *t, size_t &b) {
       return cub::DeviceRadixSort::SortPairs(t, b, g->k0.p, g->k1.p, g->v0.p, g->v1.p, (int)nc, 0, bits, s);
     });
     if (rc) return rc;
     k_vg_cand_first<<<blocks_for(nc), 256, 0, s>>>(g->k1.p, g->v1.p, nc, ncell, g->flag.p);
-    VG_CUDA(cudaGetLastError());
+    MPLB_CUDA_TRY(cudaGetLastError());
     rc = with_tmp(g, [&](void *t, size_t &b) { return cub::DeviceScan::ExclusiveSum(t, b, g->flag.p, g->pos.p, (int)nc, s); });
     if (rc) return rc;
-    k_vg_emit<<<blocks_for(nc), 256, 0, s>>>(g->flag.p, g->pos.p, g->pcell.p, nc, g->ns.p, n_ns, g->dim[0], g->dim[1], g->d_inf,
+    k_vg_emit<<<blocks_for(nc), 256, 0, s>>>(g->flag.p, g->pos.p, g->pcell.p, nc, g->ns.p, n_ns, g->dim[0], g->dim[1], g->d_inf.p,
                                              out, total, cap);
-    k_vg_add<<<blocks_for(np), 256, 0, s>>>(geo, (const char *)d_pts + i0 * 3 * (fp32 ? 4 : 8), fp32, np, g->d_map);
+    k_vg_add<<<blocks_for(np), 256, 0, s>>>(geo, (const char *)d_pts + i0 * 3 * (fp32 ? 4 : 8), fp32, np, g->d_map.p);
     mplb_internal_count_launches(9);
-    VG_CUDA(cudaGetLastError());
+    MPLB_CUDA_TRY(cudaGetLastError());
     int last[2];
-    VG_CUDA(cudaMemcpyAsync(&last[0], g->pos.p + nc - 1, sizeof(int), cudaMemcpyDeviceToHost, s));
-    VG_CUDA(cudaMemcpyAsync(&last[1], g->flag.p + nc - 1, sizeof(int), cudaMemcpyDeviceToHost, s));
-    VG_CUDA(cudaStreamSynchronize(s));
+    MPLB_CUDA_TRY(cudaMemcpyAsync(&last[0], g->pos.p + nc - 1, sizeof(int), cudaMemcpyDeviceToHost, s));
+    MPLB_CUDA_TRY(cudaMemcpyAsync(&last[1], g->flag.p + nc - 1, sizeof(int), cudaMemcpyDeviceToHost, s));
+    MPLB_CUDA_TRY(cudaStreamSynchronize(s));
     total += (long long)last[0] + last[1];
   }
   return total;
@@ -387,21 +345,21 @@ long long vg_cloud(mplb_voxel_grid *g, const int8_t *grid, const int *lo, const 
   for (int i = 0; i < 3; i++) if (up[i] <= lo[i]) return 0;
   const int bx = up[0] - lo[0], by = up[1] - lo[1];
   const long long rows = (long long)bx * by;
-  VG_CUDA(g->rows.reserve((size_t)rows + 1));
-  VG_CUDA(g->flag.reserve((size_t)rows + 1));
+  MPLB_CUDA_TRY(g->rows.reserve((size_t)rows + 1));
+  MPLB_CUDA_TRY(g->flag.reserve((size_t)rows + 1));
   k_vg_row_count<<<blocks_for(rows), 256, 0, s>>>(grid, g->dim[0], g->dim[1], lo[0], lo[1], lo[2], bx, by, up[2], g->flag.p);
-  VG_CUDA(cudaGetLastError());
-  VG_CUDA(cudaMemsetAsync(g->flag.p + rows, 0, sizeof(int), s));
+  MPLB_CUDA_TRY(cudaGetLastError());
+  MPLB_CUDA_TRY(cudaMemsetAsync(g->flag.p + rows, 0, sizeof(int), s));
   int rc = with_tmp(g, [&](void *t, size_t &b) { return cub::DeviceScan::ExclusiveSum(t, b, g->flag.p, g->rows.p, (int)rows + 1, s); });
   if (rc) return rc;
   if (out && cap > 0) {
     k_vg_row_emit<<<blocks_for(rows), 256, 0, s>>>(grid, g->geo(), lo[0], lo[1], lo[2], bx, by, up[2], g->rows.p, out, cap);
-    VG_CUDA(cudaGetLastError());
+    MPLB_CUDA_TRY(cudaGetLastError());
   }
   mplb_internal_count_launches(out && cap > 0 ? 3 : 2);
   int total = 0;
-  VG_CUDA(cudaMemcpyAsync(&total, g->rows.p + rows, sizeof(int), cudaMemcpyDeviceToHost, s));
-  VG_CUDA(cudaStreamSynchronize(s));
+  MPLB_CUDA_TRY(cudaMemcpyAsync(&total, g->rows.p + rows, sizeof(int), cudaMemcpyDeviceToHost, s));
+  MPLB_CUDA_TRY(cudaStreamSynchronize(s));
   return total;
 }
 
@@ -409,36 +367,36 @@ long long host_cloud(mplb_voxel_grid *g, const int8_t *grid, const int *lo, cons
   long long n = vg_cloud(g, grid, lo, up, nullptr, 0, 0);
   if (n <= 0 || !pts || cap <= 0) return n;
   const long long w = std::min(n, cap);
-  VG_CUDA(g->pts.reserve((size_t)w * 3));
+  MPLB_CUDA_TRY(g->pts.reserve((size_t)w * 3));
   long long rc = vg_cloud(g, grid, lo, up, g->pts.p, w, 0);
   if (rc < 0) return rc;
-  VG_CUDA(cudaMemcpy(pts, g->pts.p, (size_t)w * 3 * sizeof(double), cudaMemcpyDeviceToHost));
+  MPLB_CUDA_TRY(cudaMemcpy(pts, g->pts.p, (size_t)w * 3 * sizeof(double), cudaMemcpyDeviceToHost));
   return n;
 }
 
 int check_grid(const mplb_voxel_grid *g) {
-  if (!g) return vg_fail(MPLB_ERR_ARG, "null voxel grid");
-  if (set_device(g->device)) return vg_fail(MPLB_ERR_CUDA, "cannot select the voxel grid's device");
+  if (!g) return mplb_internal_fail(MPLB_ERR_ARG, "null voxel grid");
+  if (mplb_internal_set_device(g->device)) return mplb_internal_fail(MPLB_ERR_CUDA, "cannot select the voxel grid's device");
   return MPLB_OK;
 }
 
 int upload_cells(mplb_voxel_grid *g, const int32_t *cells3, int n) {
-  VG_CUDA(g->cells.reserve((size_t)n * 3));
-  VG_CUDA(cudaMemcpy(g->cells.p, cells3, (size_t)n * 3 * sizeof(int), cudaMemcpyHostToDevice));
+  MPLB_CUDA_TRY(g->cells.reserve((size_t)n * 3));
+  MPLB_CUDA_TRY(cudaMemcpy(g->cells.p, cells3, (size_t)n * 3 * sizeof(int), cudaMemcpyHostToDevice));
   return MPLB_OK;
 }
 
 int vg_edit(mplb_voxel_grid *g, const int32_t *cells3, int n, int column, int8_t value) {
   int rc = check_grid(g);
   if (rc) return rc;
-  if (n < 0 || (n > 0 && !cells3)) return vg_fail(MPLB_ERR_ARG, "bad cell buffer");
+  if (n < 0 || (n > 0 && !cells3)) return mplb_internal_fail(MPLB_ERR_ARG, "bad cell buffer");
   if (n == 0 || !g->ncell) return MPLB_OK;
   rc = upload_cells(g, cells3, n);
   if (rc) return rc;
-  k_vg_fill<<<(n + 255) / 256, 256>>>(g->d_map, g->cells.p, n, column, value, g->dim[0], g->dim[1], g->dim[2]);
+  k_vg_fill<<<(n + 255) / 256, 256>>>(g->d_map.p, g->cells.p, n, column, value, g->dim[0], g->dim[1], g->dim[2]);
   mplb_internal_count_launches(1);
-  VG_CUDA(cudaGetLastError());
-  VG_CUDA(cudaDeviceSynchronize());
+  MPLB_CUDA_TRY(cudaGetLastError());
+  MPLB_CUDA_TRY(cudaDeviceSynchronize());
   return MPLB_OK;
 }
 
@@ -447,37 +405,36 @@ int vg_edit(mplb_voxel_grid *g, const int32_t *cells3, int n, int column, int8_t
 extern "C" {
 
 int mplb_voxel_grid_create(const double *origin, const double *dim_m, float res, mplb_voxel_grid **out) {
-  if (!origin || !dim_m || !out) return vg_fail(MPLB_ERR_ARG, "null argument");
-  if (!(res > 0) || !std::isfinite(res)) return vg_fail(MPLB_ERR_ARG, "voxel grid resolution must be finite and > 0");
+  if (!origin || !dim_m || !out) return mplb_internal_fail(MPLB_ERR_ARG, "null argument");
+  if (!(res > 0) || !std::isfinite(res)) return mplb_internal_fail(MPLB_ERR_ARG, "voxel grid resolution must be finite and > 0");
   mplb_voxel_grid *g = new mplb_voxel_grid();
   g->res = res;
-  if (cudaGetDevice(&g->device) != cudaSuccess) { delete g; return vg_fail(MPLB_ERR_CUDA, "no CUDA device (libmplb has no CPU path)"); }
+  if (cudaGetDevice(&g->device) != cudaSuccess) { delete g; return mplb_internal_fail(MPLB_ERR_CUDA, "no CUDA device (libmplb has no CPU path)"); }
   int rc = vg_allocate(g, dim_m, origin, nullptr);
-  if (rc == MPLB_OK && cudaDeviceSynchronize() != cudaSuccess) rc = vg_fail(MPLB_ERR_CUDA, "voxel grid allocation");
-  if (rc != MPLB_OK) { g->release(); delete g; return rc; }
+  if (rc == MPLB_OK && cudaDeviceSynchronize() != cudaSuccess) rc = mplb_internal_fail(MPLB_ERR_CUDA, "voxel grid allocation");
+  if (rc != MPLB_OK) { delete g; return rc; }
   *out = g;
   return MPLB_OK;
 }
 
 void mplb_voxel_grid_destroy(mplb_voxel_grid *g) {
   if (!g) return;
-  set_device(g->device);
-  g->release();
+  mplb_internal_set_device(g->device);
   delete g;
 }
 
 int mplb_voxel_grid_allocate(mplb_voxel_grid *g, const double *dim_m, const double *origin, int32_t *changed) {
   int rc = check_grid(g);
   if (rc) return rc;
-  if (!dim_m || !origin) return vg_fail(MPLB_ERR_ARG, "null argument");
+  if (!dim_m || !origin) return mplb_internal_fail(MPLB_ERR_ARG, "null argument");
   rc = vg_allocate(g, dim_m, origin, changed);
   if (rc) return rc;
-  VG_CUDA(cudaDeviceSynchronize());
+  MPLB_CUDA_TRY(cudaDeviceSynchronize());
   return MPLB_OK;
 }
 
 int mplb_voxel_grid_get_info(const mplb_voxel_grid *g, int32_t *dim, int32_t *origin_i, double *origin_d, float *res) {
-  if (!g) return vg_fail(MPLB_ERR_ARG, "null voxel grid");
+  if (!g) return mplb_internal_fail(MPLB_ERR_ARG, "null voxel grid");
   for (int i = 0; i < 3; i++) {
     if (dim) dim[i] = g->dim[i];
     if (origin_i) origin_i[i] = g->ori[i];
@@ -491,32 +448,32 @@ int mplb_voxel_grid_clear(mplb_voxel_grid *g) {
   int rc = check_grid(g);
   if (rc) return rc;
   if (!g->ncell) return MPLB_OK;
-  VG_CUDA(cudaMemset(g->d_map, 0, g->ncell));
-  VG_CUDA(cudaMemset(g->d_inf, 0, g->ncell));
-  VG_CUDA(cudaDeviceSynchronize());
+  MPLB_CUDA_TRY(cudaMemset(g->d_map.p, 0, g->ncell));
+  MPLB_CUDA_TRY(cudaMemset(g->d_inf.p, 0, g->ncell));
+  MPLB_CUDA_TRY(cudaDeviceSynchronize());
   return MPLB_OK;
 }
 
 int mplb_voxel_grid_add_cloud_device(mplb_voxel_grid *g, const void *d_pts, int64_t n, int fp32, void *stream) {
   int rc = check_grid(g);
   if (rc) return rc;
-  if (n < 0 || (n > 0 && !d_pts)) return vg_fail(MPLB_ERR_ARG, "bad point buffer");
+  if (n < 0 || (n > 0 && !d_pts)) return mplb_internal_fail(MPLB_ERR_ARG, "bad point buffer");
   if (n == 0 || !g->ncell) return MPLB_OK;
   cudaStream_t s = (cudaStream_t)stream;
-  k_vg_add<<<blocks_for((size_t)n), 256, 0, s>>>(g->geo(), d_pts, fp32 ? 1 : 0, n, g->d_map);
+  k_vg_add<<<blocks_for((size_t)n), 256, 0, s>>>(g->geo(), d_pts, fp32 ? 1 : 0, n, g->d_map.p);
   mplb_internal_count_launches(1);
-  VG_CUDA(cudaGetLastError());
-  VG_CUDA(cudaStreamSynchronize(s));
+  MPLB_CUDA_TRY(cudaGetLastError());
+  MPLB_CUDA_TRY(cudaStreamSynchronize(s));
   return MPLB_OK;
 }
 
 int mplb_voxel_grid_add_cloud(mplb_voxel_grid *g, const double *pts, int64_t n) {
   int rc = check_grid(g);
   if (rc) return rc;
-  if (n < 0 || (n > 0 && !pts)) return vg_fail(MPLB_ERR_ARG, "bad point buffer");
+  if (n < 0 || (n > 0 && !pts)) return mplb_internal_fail(MPLB_ERR_ARG, "bad point buffer");
   if (n == 0 || !g->ncell) return MPLB_OK;
-  VG_CUDA(g->pts.reserve((size_t)n * 3));
-  VG_CUDA(cudaMemcpy(g->pts.p, pts, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice));
+  MPLB_CUDA_TRY(g->pts.reserve((size_t)n * 3));
+  MPLB_CUDA_TRY(cudaMemcpy(g->pts.p, pts, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice));
   return mplb_voxel_grid_add_cloud_device(g, g->pts.p, n, 0, nullptr);
 }
 
@@ -525,7 +482,7 @@ int64_t mplb_voxel_grid_add_cloud_inflated_device(mplb_voxel_grid *g, const void
   int rc = check_grid(g);
   if (rc) return rc;
   if (n < 0 || (n > 0 && !d_pts) || n_ns < 0 || (n_ns > 0 && !ns) || cap < 0 || (cap > 0 && !d_new_obs))
-    return vg_fail(MPLB_ERR_ARG, "bad argument");
+    return mplb_internal_fail(MPLB_ERR_ARG, "bad argument");
   return vg_add_inflated(g, d_pts, n, fp32 ? 1 : 0, ns, n_ns, (int *)d_new_obs, cap, (cudaStream_t)stream);
 }
 
@@ -534,20 +491,20 @@ int64_t mplb_voxel_grid_add_cloud_inflated(mplb_voxel_grid *g, const double *pts
   int rc = check_grid(g);
   if (rc) return rc;
   if (n < 0 || (n > 0 && !pts) || n_ns < 0 || (n_ns > 0 && !ns) || cap < 0 || (cap > 0 && !new_obs))
-    return vg_fail(MPLB_ERR_ARG, "bad argument");
+    return mplb_internal_fail(MPLB_ERR_ARG, "bad argument");
   if (n == 0) return 0;
   cap = std::min<int64_t>(cap, (int64_t)g->ncell); /* one call emits a cell at most once: the rows past ncell stay unused */
-  VG_CUDA(g->pts.reserve((size_t)n * 3));
-  VG_CUDA(cudaMemcpy(g->pts.p, pts, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice));
-  if (cap > 0) VG_CUDA(g->obs.reserve((size_t)cap * 3));
+  MPLB_CUDA_TRY(g->pts.reserve((size_t)n * 3));
+  MPLB_CUDA_TRY(cudaMemcpy(g->pts.p, pts, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice));
+  if (cap > 0) MPLB_CUDA_TRY(g->obs.reserve((size_t)cap * 3));
   const long long count = vg_add_inflated(g, g->pts.p, n, 0, ns, n_ns, g->obs.p, cap, 0);
   if (count > 0 && cap > 0)
-    VG_CUDA(cudaMemcpy(new_obs, g->obs.p, (size_t)std::min<long long>(count, cap) * 3 * sizeof(int), cudaMemcpyDeviceToHost));
+    MPLB_CUDA_TRY(cudaMemcpy(new_obs, g->obs.p, (size_t)std::min<long long>(count, cap) * 3 * sizeof(int), cudaMemcpyDeviceToHost));
   return count;
 }
 
 int mplb_voxel_grid_set_chunk_points(mplb_voxel_grid *g, int64_t points) {
-  if (!g || points < 0) return vg_fail(MPLB_ERR_ARG, "bad argument");
+  if (!g || points < 0) return mplb_internal_fail(MPLB_ERR_ARG, "bad argument");
   g->chunk_points = points;
   return MPLB_OK;
 }
@@ -556,10 +513,10 @@ int mplb_voxel_grid_decay(mplb_voxel_grid *g) {
   int rc = check_grid(g);
   if (rc) return rc;
   if (!g->ncell) return MPLB_OK;
-  k_vg_decay<<<blocks_for(g->ncell), 256>>>(g->d_map, g->d_inf, g->ncell);
+  k_vg_decay<<<blocks_for(g->ncell), 256>>>(g->d_map.p, g->d_inf.p, g->ncell);
   mplb_internal_count_launches(1);
-  VG_CUDA(cudaGetLastError());
-  VG_CUDA(cudaDeviceSynchronize());
+  MPLB_CUDA_TRY(cudaGetLastError());
+  MPLB_CUDA_TRY(cudaDeviceSynchronize());
   return MPLB_OK;
 }
 
@@ -572,16 +529,16 @@ int mplb_voxel_grid_clear_columns(mplb_voxel_grid *g, const int32_t *cells3, int
 int64_t mplb_voxel_grid_get_cloud(mplb_voxel_grid *g, double *pts, int64_t cap) {
   int rc = check_grid(g);
   if (rc) return rc;
-  if (cap < 0) return vg_fail(MPLB_ERR_ARG, "negative capacity");
+  if (cap < 0) return mplb_internal_fail(MPLB_ERR_ARG, "negative capacity");
   const int lo[3] = {0, 0, 0};
-  return host_cloud(g, g->d_map, lo, g->dim, pts, cap);
+  return host_cloud(g, g->d_map.p, lo, g->dim, pts, cap);
 }
 
 int64_t mplb_voxel_grid_get_local_cloud(mplb_voxel_grid *g, const double *pos, const double *ori, const double *dim, double *pts,
                                         int64_t cap) {
   int rc = check_grid(g);
   if (rc) return rc;
-  if (!pos || !ori || !dim || cap < 0) return vg_fail(MPLB_ERR_ARG, "bad argument");
+  if (!pos || !ori || !dim || cap < 0) return mplb_internal_fail(MPLB_ERR_ARG, "bad argument");
   int lo[3], up[3];
   for (int i = 0; i < 3; i++) { /* vg:49-55: floatToInt(pos + ori) clamped >= 0, floatToInt(pos + ori + dim) clamped <= dim_ */
     const double a = pos[i] + ori[i], b = a + dim[i];
@@ -591,71 +548,67 @@ int64_t mplb_voxel_grid_get_local_cloud(mplb_voxel_grid *g, const double *pos, c
     lo[i] = na < 0 ? 0 : na;
     up[i] = nb > g->dim[i] ? g->dim[i] : nb;
   }
-  return host_cloud(g, g->d_inf, lo, up, pts, cap);
+  return host_cloud(g, g->d_inf.p, lo, up, pts, cap);
 }
 
 int mplb_voxel_grid_get_map(mplb_voxel_grid *g, int inflated, int8_t *out, size_t cap) {
   int rc = check_grid(g);
   if (rc) return rc;
-  if (!out && g->ncell) return vg_fail(MPLB_ERR_ARG, "null output");
-  if (cap < g->ncell) return vg_fail(MPLB_ERR_ARG, "output buffer smaller than the grid");
+  if (!out && g->ncell) return mplb_internal_fail(MPLB_ERR_ARG, "null output");
+  if (cap < g->ncell) return mplb_internal_fail(MPLB_ERR_ARG, "output buffer smaller than the grid");
   if (!g->ncell) return MPLB_OK;
-  VG_CUDA(g->bytes.reserve(g->ncell));
-  k_vg_binarize<<<blocks_for(g->ncell), 256>>>(inflated ? g->d_inf : g->d_map, g->bytes.p, g->ncell);
+  MPLB_CUDA_TRY(g->bytes.reserve(g->ncell));
+  k_vg_binarize<<<blocks_for(g->ncell), 256>>>(inflated ? g->d_inf.p : g->d_map.p, g->bytes.p, g->ncell);
   mplb_internal_count_launches(1);
-  VG_CUDA(cudaGetLastError());
-  VG_CUDA(cudaMemcpy(out, g->bytes.p, g->ncell, cudaMemcpyDeviceToHost));
+  MPLB_CUDA_TRY(cudaGetLastError());
+  MPLB_CUDA_TRY(cudaMemcpy(out, g->bytes.p, g->ncell, cudaMemcpyDeviceToHost));
   return MPLB_OK;
 }
 
 int mplb_voxel_grid_write_map(mplb_voxel_grid *g, int inflated, mplb_map *m) {
   int rc = check_grid(g);
   if (rc) return rc;
-  if (!m) return vg_fail(MPLB_ERR_ARG, "null map");
+  if (!m) return mplb_internal_fail(MPLB_ERR_ARG, "null map");
   MplbMapView v;
   mplb_internal_map_view(m, &v);
   if (v.dim != 3 || v.device != g->device || v.res != (double)g->res)
-    return vg_fail(MPLB_ERR_ARG, "map is not 3D on the grid's device with the grid's resolution");
+    return mplb_internal_fail(MPLB_ERR_ARG, "map is not 3D on the grid's device with the grid's resolution");
   for (int i = 0; i < 3; i++)
-    if (v.nd[i] != g->dim[i] || v.origin[i] != g->origin_d[i]) return vg_fail(MPLB_ERR_ARG, "map geometry differs from the grid's");
-  k_vg_binarize<<<blocks_for(g->ncell), 256>>>(inflated ? g->d_inf : g->d_map, v.d_grid, g->ncell);
+    if (v.nd[i] != g->dim[i] || v.origin[i] != g->origin_d[i]) return mplb_internal_fail(MPLB_ERR_ARG, "map geometry differs from the grid's");
+  k_vg_binarize<<<blocks_for(g->ncell), 256>>>(inflated ? g->d_inf.p : g->d_map.p, v.d_grid, g->ncell);
   mplb_internal_count_launches(1);
-  VG_CUDA(cudaGetLastError());
+  MPLB_CUDA_TRY(cudaGetLastError());
   rc = mplb_internal_map_cells_changed(m, nullptr);
   if (rc) return rc;
-  VG_CUDA(cudaDeviceSynchronize());
+  MPLB_CUDA_TRY(cudaDeviceSynchronize());
   return MPLB_OK;
 }
 
 int mplb_voxel_grid_create_map(mplb_voxel_grid *g, int inflated, mplb_map **out) {
   int rc = check_grid(g);
   if (rc) return rc;
-  if (!out) return vg_fail(MPLB_ERR_ARG, "null argument");
-  if (!g->ncell) return vg_fail(MPLB_ERR_ARG, "the grid has no cells");
-  VG_CUDA(g->bytes.reserve(g->ncell));
-  k_vg_binarize<<<blocks_for(g->ncell), 256>>>(inflated ? g->d_inf : g->d_map, g->bytes.p, g->ncell);
+  if (!out) return mplb_internal_fail(MPLB_ERR_ARG, "null argument");
+  if (!g->ncell) return mplb_internal_fail(MPLB_ERR_ARG, "the grid has no cells");
+  MPLB_CUDA_TRY(g->bytes.reserve(g->ncell));
+  k_vg_binarize<<<blocks_for(g->ncell), 256>>>(inflated ? g->d_inf.p : g->d_map.p, g->bytes.p, g->ncell);
   mplb_internal_count_launches(1);
-  VG_CUDA(cudaGetLastError());
+  MPLB_CUDA_TRY(cudaGetLastError());
   return mplb_map_create_from_device(3, g->dim, g->origin_d, (double)g->res, g->bytes.p, nullptr, out);
 }
 
 int mplb_map_get_cells(const mplb_map *m, const int32_t *cells3, int n, int32_t *values) {
-  if (!m || n < 0 || (n > 0 && (!cells3 || !values))) return vg_fail(MPLB_ERR_ARG, "bad argument");
+  if (!m || n < 0 || (n > 0 && (!cells3 || !values))) return mplb_internal_fail(MPLB_ERR_ARG, "bad argument");
   if (n == 0) return MPLB_OK;
   MplbMapView v;
   mplb_internal_map_view(const_cast<mplb_map *>(m), &v);
-  if (set_device(v.device)) return vg_fail(MPLB_ERR_CUDA, "cannot select the map's device");
-  int *d = nullptr;
-  VG_CUDA(cudaMalloc((void **)&d, (size_t)n * 4 * sizeof(int)));
-  cudaError_t e = cudaMemcpy(d, cells3, (size_t)n * 3 * sizeof(int), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) {
-    k_map_get_cells<<<(n + 255) / 256, 256>>>(v.d_grid, v.dim, v.nd[0], v.nd[1], v.nd[2], d, n, d + (size_t)n * 3);
-    mplb_internal_count_launches(1);
-    e = cudaGetLastError();
-  }
-  if (e == cudaSuccess) e = cudaMemcpy(values, d + (size_t)n * 3, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost);
-  cudaFree(d);
-  if (e != cudaSuccess) return vg_fail(MPLB_ERR_CUDA, cudaGetErrorString(e));
+  if (mplb_internal_set_device(v.device)) return mplb_internal_fail(MPLB_ERR_CUDA, "cannot select the map's device");
+  DevBuf<int> d;
+  MPLB_CUDA_TRY(d.reserve((size_t)n * 4));
+  MPLB_CUDA_TRY(cudaMemcpy(d.p, cells3, (size_t)n * 3 * sizeof(int), cudaMemcpyHostToDevice));
+  k_map_get_cells<<<(n + 255) / 256, 256>>>(v.d_grid, v.dim, v.nd[0], v.nd[1], v.nd[2], d.p, n, d.p + (size_t)n * 3);
+  mplb_internal_count_launches(1);
+  MPLB_CUDA_TRY(cudaGetLastError());
+  MPLB_CUDA_TRY(cudaMemcpy(values, d.p + (size_t)n * 3, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost));
   return MPLB_OK;
 }
 

@@ -57,3 +57,21 @@ def test_product_never_imports_oracle():
             if f.endswith((".py", ".cu", ".cuh", ".h", ".hpp")):
                 src = open(os.path.join(dirpath, f)).read()
                 assert "import oracle" not in src and "oracle/" not in src and "mpl_oracle" not in src, f
+
+
+def test_device_memory_has_one_owner():
+    """Every device allocation of libmplb goes through DevBuf in mplb_internal.h, which frees what it owns, and every CUDA
+    error is reported by its one macro: no unit allocates or frees raw device memory or defines an error macro of its own."""
+    csrc = os.path.join(ROOT, "mpl_ros_b200", "csrc")
+    devbuf = 0
+    for f in sorted(os.listdir(csrc)):
+        if not f.endswith((".cu", ".cuh", ".h")):
+            continue
+        src = open(os.path.join(csrc, f)).read()
+        devbuf += len(re.findall(r"\bstruct\s+(?:\w+\s+)?DevBuf\b\s*\{", src))
+        if f == "mplb_internal.h":
+            continue
+        assert not re.search(r"\bcuda(?:Malloc|Free)\s*\(", src), f
+        for name, body in re.findall(r"#define\s+(\w+)((?:[^\n]*\\\n)*[^\n]*)", src):
+            assert not re.search(r"\bcudaError_t\b|\bcudaGetErrorString\b", body), (f, name)
+    assert devbuf == 1
