@@ -299,8 +299,11 @@ int mplb_refine_trajectories(mplb_planner *p, const mplb_result *results, const 
 
 /* ---- LPA* incremental replanning (SURVEY section 8f.3; mpl_test_node/src/map_replanner_node.cpp:107-241 is the caller).
  * The search state of a planner with LPA* enabled stays on the device between plans; each call below is the member of the
- * same name.  Plain occupancy maps only: a potential map, a search region, a prior trajectory or yaw controls make
- * mplb_plan fail with MPLB_ERR_ARG while LPA* is on.  Where the reference iterates its hash map (getSubStateSpace re-pushing
+ * same name.  Occupancy maps with or without a potential map (mplb_planner_set_potential_map /
+ * mplb_planner_update_potential_map, MPLB_POTENTIAL_WEIGHT / MPLB_GRADIENT_WEIGHT) and the *xYAW controls (control rows of
+ * Dim + 1 entries, MPLB_YAW_MAX / MPLB_WYAW) replan like the plain map; a search region or a prior trajectory makes mplb_plan
+ * fail with MPLB_ERR_ARG while LPA* is on.  Stored edge costs are never recomputed when the potential map is replaced, and
+ * updateClearedNodes restores an edge as J + w dt without potential or heading terms, both as the reference.  Where the reference iterates its hash map (getSubStateSpace re-pushing
  * the open set, getLinkedNodes filling the voxel -> edge lists) the order is INSERTION order; Boost leaves it unspecified, and
  * it only decides the order among exact key ties (DESIGN.md section 4.12). */
 /* PlannerBase::setLPAstar (planner_base.h:170-176): from now on mplb_plan runs GraphSearch::LPAstar (graph_search.h:194-365)

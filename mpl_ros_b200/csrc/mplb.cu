@@ -1059,8 +1059,10 @@ int mplb_internal_planner_cfg(mplb_planner *p, MplbLpaHostCfg *o) {
   o->lpa_init_nodes = p->lpa_init_nodes; o->lpa_init_preds = p->lpa_init_preds;
   o->U = p->U.data();
   o->Uyaw = p->Uyaw.empty() ? nullptr : p->Uyaw.data();
-  o->shaped = (p->pot_cells != 0 || !p->h_region.empty() || p->prior_nseg != 0 || !p->Uyaw.empty()) ? 1 : 0;
+  o->astar_only = (!p->h_region.empty() || p->prior_nseg != 0) ? 1 : 0;
+  o->pot_w = p->pot_w; o->grad_w = p->grad_w; o->wyaw = p->wyaw; o->yaw_max = p->yaw_max;
   o->has_map = p->map != nullptr;
+  if (p->pot_cells) { o->d_pot = p->d_pot.p; o->pot_cells = p->pot_cells; }
   if (p->map) {
     for (int i = 0; i < 3; i++) { o->nd[i] = p->map->nd[i]; o->origin[i] = p->map->origin[i]; }
     o->res = p->map->res;

@@ -79,7 +79,7 @@ struct mplb_result;
 struct mplb_waypoint;
 struct MplbLpaHostCfg {
   int dim, nU, max_num, device, verbose, has_map;
-  int shaped; /* potential map / search region / prior trajectory / yaw controls installed: not available under LPA* */
+  int astar_only; /* search region / prior trajectory installed: not available under LPA* */
   int lpa_init_nodes, lpa_init_preds; /* MPLB_LPA_INIT_NODES / MPLB_LPA_INIT_PREDS */
   double v_max, a_max, j_max, dt, w, eps, tol_pos, tol_vel, tol_acc;
   int nd[3];
@@ -88,6 +88,9 @@ struct MplbLpaHostCfg {
   const int8_t *d_grid; /* the map's int8 cells on the planner's device */
   const double *U;      /* host, nU rows of 3 */
   const double *Uyaw;   /* host, nU yaw rates, or NULL when the control rows carry none */
+  const int8_t *d_pot;  /* the planner's potential map on its device, or NULL */
+  size_t pot_cells;     /* its entries (one per map cell when it matches the map) */
+  double pot_w, grad_w, wyaw, yaw_max;
 };
 MPLB_HIDDEN int mplb_internal_planner_cfg(mplb_planner *p, MplbLpaHostCfg *out);
 /* the retained single plan the getters mplb_get_actions / mplb_get_seg_states serve */

@@ -12,6 +12,8 @@
  *   k_lpa_plan        the LPA* loop; 32 lanes generate the |U| successor rows of a popped node and then share its graph update
  *                     (key-table probes, new States, predecessor appends, rhs recomputation); lane 0 keeps what defines order:
  *                     ids, iteration-order slots and the priority-queue operations
+ *   k_lpa_plan_shaped the same loop for sessions with a potential map or yaw controls (the SH statements of the core); a batch
+ *                     that mixes kinds is one launch per kind on the same stream
  *   k_lpa_subtree     getSubStateSpace (a Dijkstra-like sweep over stored successor lists, serial by nature)
  *   k_lpa_link_count / k_lpa_link_scan / k_lpa_link_fill    the voxel -> edge table in insertion order (count, scan, fill)
  *   k_lpa_match       one thread per link against the changed voxels;  k_lpa_apply  sort + increaseCost / decreaseCost
@@ -44,8 +46,9 @@ __device__ void wp_to_state(const mplb_waypoint &w, double *st) {
   st[12] = w.yaw;
 }
 
-__global__ void __launch_bounds__(32)
-k_lpa_plan(Ctx *ctxs, const mplb_waypoint *starts, const mplb_waypoint *goals, mplb_result *results, int *acts, double *segs, int max_seg) {
+template <bool SH>
+__device__ __forceinline__ void lpa_plan_body(Ctx *ctxs, const mplb_waypoint *starts, const mplb_waypoint *goals, mplb_result *results,
+                                              int *acts, double *segs, int max_seg) {
   __shared__ Ctx x;
   __shared__ int s_code;
   __shared__ PopScratch s_pop;
@@ -58,7 +61,7 @@ k_lpa_plan(Ctx *ctxs, const mplb_waypoint *starts, const mplb_waypoint *goals, m
       double sst[13], gst[13];
       wp_to_state(starts[b], sst);
       wp_to_state(goals[b], gst);
-      st = plan_begin(x, sst, starts[b].t, gst);
+      st = plan_begin<SH>(x, sst, starts[b].t, gst);
     }
     s_code = st;
   }
@@ -73,17 +76,17 @@ k_lpa_plan(Ctx *ctxs, const mplb_waypoint *starts, const mplb_waypoint *goals, m
     __syncwarp();
     if (r == -1) { /* one lane per control: end state, validation, lattice key, collision samples */
       const Node &n = x.nodes[x.h->curr];
-      for (int u = lane; u < nU; u += 32) succ_row(x.cfg, n.st, n.t, n.key, u, &x.rows[u]);
+      for (int u = lane; u < nU; u += 32) succ_row<SH>(x.cfg, x.h->sh, n.st, n.t, n.key, u, &x.rows[u]);
       __syncwarp();
     }
     if (r == -1 || r == -2) {
 #ifdef MPLB_LPA_SERIAL_FINISH /* the one-lane tail, kept for A/B runs */
-      if (lane == 0) s_code = pop_finish(x);
+      if (lane == 0) s_code = pop_finish<SH>(x);
       __syncwarp();
       code = s_code;
       __syncwarp();
 #else /* probes, new States, predecessor appends and rhs over the lanes; ids, slots and queue operations on lane 0 */
-      pop_finish_warp(x, &s_pop);
+      pop_finish_warp<SH>(x, &s_pop);
       code = s_pop.ret;
       __syncwarp();
 #endif
@@ -135,6 +138,18 @@ k_lpa_plan(Ctx *ctxs, const mplb_waypoint *starts, const mplb_waypoint *goals, m
     r.pop_hash = have_state ? h.pop_hash : 0;
     results[b] = r;
   }
+}
+
+/* plain occupancy map: the statements without the potential / yaw branches */
+__global__ void __launch_bounds__(32)
+k_lpa_plan(Ctx *ctxs, const mplb_waypoint *starts, const mplb_waypoint *goals, mplb_result *results, int *acts, double *segs, int max_seg) {
+  lpa_plan_body<false>(ctxs, starts, goals, results, acts, segs, max_seg);
+}
+/* potential map and / or yaw controls (Hdr::sh) */
+__global__ void __launch_bounds__(32)
+k_lpa_plan_shaped(Ctx *ctxs, const mplb_waypoint *starts, const mplb_waypoint *goals, mplb_result *results, int *acts, double *segs,
+                  int max_seg) {
+  lpa_plan_body<true>(ctxs, starts, goals, results, acts, segs, max_seg);
 }
 
 __global__ void __launch_bounds__(32) k_lpa_subtree(Ctx *ctxs, int time_step) {
@@ -224,7 +239,7 @@ struct Session {
   DevBuf<Succ> succ;
   DevBuf<Pred> preds;
   DevBuf<int> table, order, order2, heap_node, best, traj_act, epq_node, link_count, cells;
-  DevBuf<double> heap_f, epq_f, U, segs;
+  DevBuf<double> heap_f, epq_f, U, Uyaw, segs;
   DevBuf<Row> rows;
   DevBuf<unsigned char> mark;
   DevBuf<Link> links;
@@ -236,6 +251,8 @@ struct Session {
   int init_nodes = 1 << 16, init_pred = 1 << 20; /* MPLB_LPA_INIT_NODES / _PREDS, read at every plan, used when allocating */
   int grows = 0;                                 /* doublings since the arrays were allocated */
   bool have_links = false;
+  bool shaped = false; /* potential map or yaw controls: planned by k_lpa_plan_shaped with `sh` in its header */
+  Shape sh{};
 };
 
 std::unordered_map<mplb_planner *, Session *> g_sessions; /* planner -> its replanning session; the registry is locked, a
@@ -319,8 +336,15 @@ int refresh_cfg(mplb_planner *p, Session *s, int control) {
   if (!hc.has_map) return mplb_internal_fail(MPLB_ERR_STATE, "LPA*: no map set");
   if (hc.nU <= 0) return mplb_internal_fail(MPLB_ERR_STATE, "LPA*: no controls set");
   if (hc.nU > LPA_MAXU) return mplb_internal_fail(MPLB_ERR_ARG, "LPA*: more than 128 controls");
-  if (hc.shaped) return mplb_internal_fail(MPLB_ERR_ARG, "LPA*: potential map / search region / prior trajectory / yaw controls are A*-only on this path");
-  if (control & 16) return mplb_internal_fail(MPLB_ERR_ARG, "LPA*: yaw controls are A*-only on this path");
+  if (hc.astar_only) return mplb_internal_fail(MPLB_ERR_ARG, "LPA*: search region / prior trajectory are A*-only on this path");
+  if (control & ~31) return mplb_internal_fail(MPLB_ERR_ARG, "LPA*: unsupported control flag on the start waypoint");
+  const bool yaw = (control & 16) != 0;
+  if (yaw && !hc.Uyaw)
+    return mplb_internal_fail(MPLB_ERR_ARG, "LPA*: the start waypoint uses yaw but the control rows have no yaw column (setU rows need Dim + 1 entries)");
+  if (yaw && hc.dim < 2) return mplb_internal_fail(MPLB_ERR_ARG, "LPA*: yaw controls need a planar velocity (Dim >= 2)");
+  if (yaw && hc.yaw_max > 0 && !(hc.yaw_max < 1e5)) return mplb_internal_fail(MPLB_ERR_ARG, "LPA*: yaw_max is out of range");
+  if (hc.d_pot && hc.pot_cells != (size_t)hc.nd[0] * hc.nd[1] * (hc.dim == 3 ? hc.nd[2] : 1))
+    return mplb_internal_fail(MPLB_ERR_STATE, "LPA*: potential map size does not match the planner's map");
   const int cc = control & 15;
   const int ord = cc == 1 ? 1 : cc == 3 ? 2 : cc == 7 ? 3 : cc == 15 ? 4 : 0;
   if (!ord) return mplb_internal_fail(MPLB_ERR_ARG, "LPA*: the start waypoint carries no control flag");
@@ -332,8 +356,20 @@ int refresh_cfg(mplb_planner *p, Session *s, int control) {
   s->init_nodes = hc.lpa_init_nodes; s->init_pred = hc.lpa_init_preds;
   MPLB_CUDA_TRY(s->U.grow((size_t)hc.nU * 3, 0));
   MPLB_CUDA_TRY(cudaMemcpy(s->U.p, hc.U, (size_t)hc.nU * 3 * sizeof(double), cudaMemcpyHostToDevice));
+  /* cost shaping and yaw (em:104-128, pr:503-525): the planner's device copy of its potential map, the yaw column of U */
+  Shape &sh = s->sh;
+  sh = Shape{};
+  sh.pot = hc.d_pot; sh.pot_w = hc.pot_w; sh.grad_w = hc.grad_w;
+  sh.use_yaw = yaw ? 1 : 0; sh.wyaw = hc.wyaw; sh.yaw_max = hc.yaw_max; sh.cos_yaw_max = 1.0;
+  if (yaw) {
+    MPLB_CUDA_TRY(s->Uyaw.grow((size_t)hc.nU, 0));
+    MPLB_CUDA_TRY(cudaMemcpy(s->Uyaw.p, hc.Uyaw, (size_t)hc.nU * sizeof(double), cudaMemcpyHostToDevice));
+    sh.Uyaw = s->Uyaw.p;
+    if (hc.yaw_max > 0) { double sn; mplb::trig::sincos_cr(hc.yaw_max, &sn, &sh.cos_yaw_max); } /* cos(my) of pr:521 */
+  }
+  s->shaped = sh.pot != nullptr || yaw;
   Cfg &c = s->h.cfg;
-  c.dim = hc.dim; c.ord = ord; c.control = control; c.nU = hc.nU; c.nkey = hc.dim * ord; c.max_num = hc.max_num;
+  c.dim = hc.dim; c.ord = ord; c.control = control; c.nU = hc.nU; c.nkey = hc.dim * ord + (yaw ? 1 : 0); c.max_num = hc.max_num;
   c.dt = hc.dt; c.w = hc.w; c.eps = hc.eps; c.v_max = hc.v_max; c.a_max = hc.a_max; c.j_max = hc.j_max;
   c.tol_pos = hc.tol_pos; c.tol_vel = hc.tol_vel; c.tol_acc = hc.tol_acc;
   for (int i = 0; i < 3; i++) { c.nd[i] = hc.nd[i]; c.origin[i] = hc.origin[i]; }
@@ -374,24 +410,47 @@ int plan_sessions(std::vector<mplb_planner *> &ps, const mplb_waypoint *starts, 
     if (rc) return rc;
     if (hd.n_nodes + 1 > s->cap_nodes) { rc = grow_session(s); if (rc) return rc; }
   }
-  /* the batch's contexts, contiguous */
+  /* the batch's contexts, contiguous: the plain sessions first, then the shaped ones, so that each kind is one launch over a
+     contiguous range of slots; slot[i] is planner i's position */
   Session *lead = ss[0];
   const int max_seg = 4096; /* per-plan trajectory rows of the launch; longer trajectories are gathered after it */
+  std::vector<int> slot(n);
+  int n_plain = 0;
+  for (int i = 0; i < n; i++) if (!ss[i]->shaped) slot[i] = n_plain++;
+  for (int i = 0, k = n_plain; i < n; i++) if (ss[i]->shaped) slot[i] = k++;
+  std::vector<mplb_waypoint> wps(2 * (size_t)n);
+  for (int i = 0; i < n; i++) { wps[slot[i]] = starts[i]; wps[n + slot[i]] = goals[i]; }
   DevBuf<Ctx> ctxs;
   MPLB_CUDA_TRY(ctxs.grow(n, 0));
-  for (int i = 0; i < n; i++) MPLB_CUDA_TRY(cudaMemcpy(ctxs.p + i, &ss[i]->h, sizeof(Ctx), cudaMemcpyHostToDevice));
+  for (int i = 0; i < n; i++) MPLB_CUDA_TRY(cudaMemcpy(ctxs.p + slot[i], &ss[i]->h, sizeof(Ctx), cudaMemcpyHostToDevice));
   MPLB_CUDA_TRY(lead->wps.grow((size_t)2 * n, 0));
   MPLB_CUDA_TRY(lead->res.grow(n, 0));
   MPLB_CUDA_TRY(lead->acts.grow((size_t)n * max_seg, 0));
   MPLB_CUDA_TRY(lead->segs.grow((size_t)n * max_seg * 13, 0));
-  MPLB_CUDA_TRY(cudaMemcpy(lead->wps.p, starts, (size_t)n * sizeof(mplb_waypoint), cudaMemcpyHostToDevice));
-  MPLB_CUDA_TRY(cudaMemcpy(lead->wps.p + n, goals, (size_t)n * sizeof(mplb_waypoint), cudaMemcpyHostToDevice));
-  for (int i = 0; i < n; i++) { Hdr hd; int rc = read_hdr(ss[i], &hd); if (rc) return rc; hd.resume = 0; hd.status = 0; rc = write_hdr(ss[i], hd); if (rc) return rc; }
+  MPLB_CUDA_TRY(cudaMemcpy(lead->wps.p, wps.data(), (size_t)2 * n * sizeof(mplb_waypoint), cudaMemcpyHostToDevice));
+  for (int i = 0; i < n; i++) {
+    Hdr hd;
+    int rc = read_hdr(ss[i], &hd);
+    if (rc) return rc;
+    hd.resume = 0; hd.status = 0; hd.sh = ss[i]->sh;
+    rc = write_hdr(ss[i], hd);
+    if (rc) return rc;
+  }
   /* every round doubles the arrays of the sessions that stopped, so 64 rounds cannot run out before int capacities do */
+  const int n_shaped = n - n_plain;
   for (int round = 0; round < 64; round++) {
-    k_lpa_plan<<<n, 32>>>(ctxs.p, lead->wps.p, lead->wps.p + n, lead->res.p, lead->acts.p, lead->segs.p, max_seg);
-    mplb_internal_count_launches(1);
-    MPLB_CUDA_TRY(cudaGetLastError());
+    const mplb_waypoint *d_s = lead->wps.p, *d_g = lead->wps.p + n;
+    if (n_plain > 0) {
+      k_lpa_plan<<<n_plain, 32>>>(ctxs.p, d_s, d_g, lead->res.p, lead->acts.p, lead->segs.p, max_seg);
+      mplb_internal_count_launches(1);
+      MPLB_CUDA_TRY(cudaGetLastError());
+    }
+    if (n_shaped > 0) {
+      k_lpa_plan_shaped<<<n_shaped, 32>>>(ctxs.p + n_plain, d_s + n_plain, d_g + n_plain, lead->res.p + n_plain,
+                                          lead->acts.p + (size_t)n_plain * max_seg, lead->segs.p + (size_t)n_plain * max_seg * 13, max_seg);
+      mplb_internal_count_launches(1);
+      MPLB_CUDA_TRY(cudaGetLastError());
+    }
     MPLB_CUDA_TRY(cudaDeviceSynchronize());
     bool again = false;
     for (int i = 0; i < n; i++) {
@@ -401,13 +460,15 @@ int plan_sessions(std::vector<mplb_planner *> &ps, const mplb_waypoint *starts, 
       if (hd.status == LPA_NEED_GROW) { /* stopped before a pop that could overflow: double and resume */
         rc = grow_session(ss[i]);
         if (rc) return rc;
-        MPLB_CUDA_TRY(cudaMemcpy(ctxs.p + i, &ss[i]->h, sizeof(Ctx), cudaMemcpyHostToDevice));
+        MPLB_CUDA_TRY(cudaMemcpy(ctxs.p + slot[i], &ss[i]->h, sizeof(Ctx), cudaMemcpyHostToDevice));
         again = true;
       }
     }
     if (!again) break;
   }
-  MPLB_CUDA_TRY(cudaMemcpy(results, lead->res.p, (size_t)n * sizeof(mplb_result), cudaMemcpyDeviceToHost));
+  std::vector<mplb_result> res_slots(n);
+  MPLB_CUDA_TRY(cudaMemcpy(res_slots.data(), lead->res.p, (size_t)n * sizeof(mplb_result), cudaMemcpyDeviceToHost));
+  for (int i = 0; i < n; i++) results[i] = res_slots[slot[i]];
   std::vector<int> acts;
   std::vector<double> segs;
   for (int i = 0; i < n; i++) { /* retained trajectory for mplb_get_actions / mplb_get_seg_states (traj_ stays as it was on failure) */
@@ -416,14 +477,14 @@ int plan_sessions(std::vector<mplb_planner *> &ps, const mplb_waypoint *starts, 
     const int ns = results[i].n_seg;
     acts.resize(std::max(ns, 1));
     segs.resize((size_t)std::max(ns, 1) * 13);
-    const int *d_acts = lead->acts.p + (size_t)i * max_seg;
-    const double *d_segs = lead->segs.p + (size_t)i * max_seg * 13;
+    const int *d_acts = lead->acts.p + (size_t)slot[i] * max_seg;
+    const double *d_segs = lead->segs.p + (size_t)slot[i] * max_seg * 13;
     DevBuf<int> long_acts;
     DevBuf<double> long_segs;
     if (ns > max_seg) { /* the launch kept max_seg rows; traj_act / best on the device still hold the whole trajectory */
       MPLB_CUDA_TRY(long_acts.grow(ns, 0));
       MPLB_CUDA_TRY(long_segs.grow((size_t)ns * 13, 0));
-      k_lpa_traj<<<(ns + 127) / 128, 128>>>(ctxs.p + i, ns, long_acts.p, long_segs.p);
+      k_lpa_traj<<<(ns + 127) / 128, 128>>>(ctxs.p + slot[i], ns, long_acts.p, long_segs.p);
       mplb_internal_count_launches(1);
       MPLB_CUDA_TRY(cudaGetLastError());
       d_acts = long_acts.p;

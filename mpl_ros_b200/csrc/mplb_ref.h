@@ -71,6 +71,14 @@ MPLB_HD double normalize_angle(double a) { /* mt:15-19 */
   while (a < -3.141592653589793) a = dadd(a, 6.283185307179586);
   return a;
 }
+/* v.normalized().dot(Vec2f(cos yaw, sin yaw)) (pr:520, em:125): Eigen normalized() = v / sqrt(squaredNorm); cs, sn are the
+ * correctly rounded cos / sin of the yaw (mplb_trig.cuh).  sqrt is IEEE-rounded in both builds. */
+MPLB_HD double heading_dot(double vx, double vy, double cs, double sn) {
+  const double z = dadd(dmul(vx, vx), dmul(vy, vy));
+  double nx = vx, ny = vy;
+  if (z > 0.0) { const double q = sqrt(z); nx = ddiv(vx, q); ny = ddiv(vy, q); }
+  return dadd(dmul(nx, cs), dmul(ny, sn));
+}
 
 /* ------------------------------------------------------------------ Primitive1D (pr:21-198): c[0..5] = c0 .. c5 */
 struct Prim1 { double c[6]; };

@@ -625,13 +625,7 @@ __device__ __forceinline__ int sample_divisor(double max_v, double T, double res
 }
 
 /* ---------------------------------------------------------------- yaw controls (Control::*xYAW) */
-/* v.normalized().dot(Vec2f(cos yaw, sin yaw)) (pr:520, em:125): Eigen normalized() = v / sqrt(squaredNorm) */
-__device__ __forceinline__ double heading_dot(double vx, double vy, double cs, double sn) {
-  const double z = dadd(dmul(vx, vx), dmul(vy, vy));
-  double nx = vx, ny = vy;
-  if (z > 0.0) { const double q = sqrt(z); nx = ddiv(vx, q); ny = ddiv(vy, q); }
-  return dadd(dmul(nx, cs), dmul(ny, sn));
-}
+using mplb_ref::heading_dot; /* v.normalized() . (cos yaw, sin yaw), shared with the LPA* core */
 /* Lattice ints of a full state row: polynomial part (wp:95-112) and, with yaw controls, round(yaw / 0.1) (wp:114-117);
  * the yaw slot of a non-yaw plan packs as 0. */
 template <int DIM, int ORD, int NS>

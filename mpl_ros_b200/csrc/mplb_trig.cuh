@@ -10,7 +10,19 @@
  */
 #pragma once
 #include <cmath>
+#if defined(__CUDACC__)
 #include <cuda_runtime.h>
+#else /* a plain host compiler (the host build of the LPA* core, tests/cpp/lpa_emul.cpp): the qualifiers mean host code */
+#ifndef __host__
+#define __host__
+#endif
+#ifndef __device__
+#define __device__
+#endif
+#ifndef __noinline__
+#define __noinline__ __attribute__((noinline))
+#endif
+#endif
 
 namespace mplb {
 namespace trig {
