@@ -397,6 +397,29 @@ class MapUtil {
     }
     return pns;
   }
+  /* rayTrace of many rays and the replanner node's cell selection on the GPU (mplb_map_trace_cells): for every traced cell pn
+   * of ray i (p1s[i] -> p2s[i]) and every offset of `ns` (empty: the offset 0), pn + ns[k] when `select` (MPLB_TRACE_ALL /
+   * _FREE / _OCCUPIED) keeps it; `offsets` (may be NULL) receives n + 1 entries, ray i owning cells offsets[i] .. offsets[i+1]-1 */
+  vec_Veci<Dim> traceCells(const vec_Vecf<Dim> &p1s, const vec_Vecf<Dim> &p2s, const vec_Veci<Dim> &ns = vec_Veci<Dim>(),
+                           int select = MPLB_TRACE_ALL, std::vector<int64_t> *offsets = nullptr) {
+    vec_Veci<Dim> out;
+    const size_t n = std::min(p1s.size(), p2s.size());
+    std::vector<double> a(n * 3, 0.0), b(n * 3, 0.0);
+    std::vector<int32_t> s3(ns.size() * 3, 0);
+    for (size_t i = 0; i < n; i++) for (int k = 0; k < Dim; k++) { a[i * 3 + k] = p1s[i](k); b[i * 3 + k] = p2s[i](k); }
+    for (size_t i = 0; i < ns.size(); i++) for (int k = 0; k < Dim; k++) s3[i * 3 + k] = ns[i](k);
+    std::vector<int64_t> off(n + 1, 0);
+    if (!h_) return out;
+    const int64_t total = mplb_map_trace_cells(h_, a.data(), b.data(), (int)n, s3.empty() ? nullptr : s3.data(), (int)ns.size(), select,
+                                               nullptr, 0, off.data());
+    if (total < 0) { std::printf("[MapUtil] traceCells failed: %s\n", mplb_last_error()); return out; }
+    std::vector<int32_t> c3((size_t)(total > 0 ? total : 1) * 3);
+    mplb_map_trace_cells(h_, a.data(), b.data(), (int)n, s3.empty() ? nullptr : s3.data(), (int)ns.size(), select, c3.data(), total,
+                         off.data());
+    for (int64_t r = 0; r < total; r++) { Veci<Dim> pn; for (int k = 0; k < Dim; k++) pn(k) = c3[r * 3 + k]; out.push_back(pn); }
+    if (offsets) *offsets = off;
+    return out;
+  }
   /* isFree / isOccupied / isUnknown by coordinate (map_util.h:57-80): outside is none of them */
   bool isFree(const Veci<Dim> &pn) { const int v = cell(pn); return v >= 0 && v < 100; }
   bool isOccupied(const Veci<Dim> &pn) { return cell(pn) == 100; }
@@ -503,6 +526,66 @@ class MapPlanner {
      * start-not-free (planner_base.h:283-287), start-is-goal (graph_search.h:44), MaxExpandStep and the empty queue
      * (graph_search.h:149-161) leave the previous trajectory in place. */
     if (!h_ || mplb_plan(h_, &s, &g, &last_) != MPLB_OK) { report(); traj_cost_ = std::numeric_limits<decimal_t>::infinity(); return false; }
+    return planned();
+  }
+
+  /* ---- fleets: one library call per replan step for many LPA* replanners (mplb_lpa_plan_batch and the mplb_lpa_*_batch
+   * calls).  Entry i leaves planners[i] exactly as the single member would; a call returns false (message printed by the first
+   * planner when it is verbose) when the library refused it, in which case no planner changed. */
+  static bool planLPABatch(const std::vector<MapPlanner *> &planners, const vec_E<Coord> &starts, const vec_E<Coord> &goals,
+                           std::vector<bool> *ok = nullptr) {
+    const size_t n = planners.size();
+    std::vector<mplb_planner *> h(n);
+    std::vector<mplb_waypoint> s(n), g(n);
+    std::vector<mplb_result> res(n > 0 ? n : 1);
+    for (size_t i = 0; i < n; i++) {
+      MapPlanner *p = planners[i];
+      if (p->h_ && p->map_util_ && p->map_util_->handle() != p->bound_map_) p->setMapUtil(p->map_util_);
+      h[i] = p->h_; s[i] = to_c(starts[i]); g[i] = to_c(goals[i]);
+    }
+    if (mplb_lpa_plan_batch(h.data(), (int)n, s.data(), g.data(), res.data()) != MPLB_OK) return batch_failed(planners);
+    if (ok) ok->assign(n, false);
+    for (size_t i = 0; i < n; i++) {
+      MapPlanner *p = planners[i];
+      p->control_ = starts[i].control;
+      p->last_ = res[i];
+      const bool r = p->planned();
+      if (ok) (*ok)[i] = r;
+    }
+    return true;
+  }
+  static std::vector<vec_Vecf<Dim>> getLinkedNodesBatch(const std::vector<MapPlanner *> &planners) {
+    const size_t n = planners.size();
+    std::vector<vec_Vecf<Dim>> out(n);
+    std::vector<mplb_planner *> h = handles(planners);
+    std::vector<int32_t> counts(n > 0 ? n : 1, 0);
+    if (mplb_lpa_get_linked_nodes_batch(h.data(), (int)n, counts.data(), nullptr, 0) != MPLB_OK) { batch_failed(planners); return out; }
+    int64_t total = 0;
+    for (size_t i = 0; i < n; i++) total += counts[i];
+    std::vector<double> p3((size_t)(total > 0 ? total : 1) * 3);
+    if (mplb_lpa_get_linked_nodes_batch(h.data(), (int)n, counts.data(), p3.data(), total) != MPLB_OK) { batch_failed(planners); return out; }
+    size_t r = 0;
+    for (size_t i = 0; i < n; i++)
+      for (int j = 0; j < counts[i]; j++, r++) { Vecf<Dim> q; for (int k = 0; k < Dim; k++) q(k) = p3[r * 3 + k]; out[i].push_back(q); }
+    return out;
+  }
+  static bool updateBlockedNodesBatch(const std::vector<MapPlanner *> &planners, const std::vector<vec_Veci<Dim>> &cells) {
+    return update_batch(planners, cells, true);
+  }
+  static bool updateClearedNodesBatch(const std::vector<MapPlanner *> &planners, const std::vector<vec_Veci<Dim>> &cells) {
+    return update_batch(planners, cells, false);
+  }
+  static bool getSubStateSpaceBatch(const std::vector<MapPlanner *> &planners, const std::vector<int> &time_steps) {
+    const size_t n = planners.size();
+    std::vector<mplb_planner *> h = handles(planners);
+    std::vector<int32_t> ts(time_steps.begin(), time_steps.end()), sizes(n > 0 ? n : 1, 0);
+    if (ts.empty()) ts.push_back(0);
+    return mplb_lpa_sub_state_space_batch(h.data(), (int)n, ts.data(), sizes.data()) == MPLB_OK || batch_failed(planners);
+  }
+
+ private:
+  /* plan()'s bookkeeping after the library planned into last_ */
+  bool planned() {
     initialized_ = true;
     traj_cost_ = last_.cost;
     if (last_.status == MPLB_PLAN_OK) {
@@ -521,6 +604,29 @@ class MapPlanner {
     } else if (last_.status == MPLB_PLAN_TRACEBACK_FAILED) traj_ = Trajectory<Dim>();
     return last_.status == MPLB_PLAN_OK || last_.status == MPLB_PLAN_START_IS_GOAL;
   }
+  static std::vector<mplb_planner *> handles(const std::vector<MapPlanner *> &planners) {
+    std::vector<mplb_planner *> h(planners.size() > 0 ? planners.size() : 1, nullptr);
+    for (size_t i = 0; i < planners.size(); i++) h[i] = planners[i]->h_;
+    return h;
+  }
+  static bool batch_failed(const std::vector<MapPlanner *> &planners) {
+    if (!planners.empty()) planners[0]->report();
+    return false;
+  }
+  static bool update_batch(const std::vector<MapPlanner *> &planners, const std::vector<vec_Veci<Dim>> &cells, bool blocked) {
+    const size_t n = planners.size();
+    std::vector<mplb_planner *> h = handles(planners);
+    std::vector<int64_t> off(n + 1, 0);
+    std::vector<int32_t> c3, visited(n > 0 ? n : 1, 0);
+    for (size_t i = 0; i < n; i++) {
+      for (const auto &pn : cells[i]) for (int k = 0; k < 3; k++) c3.push_back(k < Dim ? pn(k) : 0);
+      off[i + 1] = off[i] + (int64_t)cells[i].size();
+    }
+    return mplb_lpa_update_nodes_batch(h.data(), (int)n, blocked ? 1 : 0, c3.empty() ? nullptr : c3.data(), off.data(),
+                                       visited.data()) == MPLB_OK || batch_failed(planners);
+  }
+
+ public:
 
   Trajectory<Dim> getTraj() const { return traj_; }          /* planner_base.h:28 */
   decimal_t getTrajCost() const { return traj_cost_; }       /* planner_base.h:155 */

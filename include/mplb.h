@@ -318,6 +318,9 @@ int mplb_planner_reset(mplb_planner *p);
  * n cells (rows of 3 ints, the third ignored in 2D) receive `value`; cells outside the grid are ignored; the occupancy bit-bricks are
  * rebuilt. */
 int mplb_map_set_cells(mplb_map *m, const int32_t *cells3, int n, int value);
+/* Same with the n cell rows in device memory, read on `stream` (a cudaStream_t as void*, NULL = default); returns once the
+ * cells and the bricks are written. */
+int mplb_map_set_cells_device(mplb_map *m, const void *d_cells3, int n, int value, void *stream);
 /* MapUtil::setMap again on a map of unchanged geometry: the whole int8 grid is replaced in place, so planners that share the
  * map (setMapUtil keeps a shared pointer in the reference) see the new cells without being re-pointed. */
 int mplb_map_set_data(mplb_map *m, const int8_t *data);
@@ -337,6 +340,26 @@ int mplb_update_cleared_nodes(mplb_planner *p, const int32_t *cells3, int n);
  * trajectory of any length for mplb_get_actions / mplb_get_seg_states.  A session that has to grow stops before the pop that
  * could overflow; the host doubles its arrays and relaunches the batch, in which finished sessions return at once. */
 int mplb_lpa_plan_batch(mplb_planner **planners, int n, const mplb_waypoint *starts, const mplb_waypoint *goals, mplb_result *results);
+/* The rest of a replan cycle for many replanners per call.  Entry i leaves planners[i] exactly as the single call of the same
+ * member would, and reports what that call returns.  Every call checks all of its arguments first and fails with no planner
+ * touched when one is null, a planner appears twice, a planner has LPA* off or has not planned, the planners live on
+ * different devices, or (sub_state_space) a time step is out of range.  The kernels take one session per block over a
+ * contiguous context array, so the launches and synchronisations of a call do not grow with n (DESIGN.md section 4.12.2).
+ *   get_linked_nodes_batch      MapPlanner::getLinkedNodes (map_planner.cpp:125-158) per entry: counts[i] = its linked points;
+ *                               pts3 (may be NULL) receives the first `cap` rows of all points, entry 0's first
+ *   update_nodes_batch          updateBlockedNodes (blocked = 1) / updateClearedNodes (blocked = 0), map_planner.cpp:160-185:
+ *                               entry i's cells are rows offsets[i] .. offsets[i+1]-1 of cells3 (rows of 3 ints; offsets has
+ *                               n + 1 entries, an empty range is allowed); visited[i] = the pairs it visited
+ *   update_nodes_batch_device   the same with the cell rows in device memory (offsets and visited stay host arrays)
+ *   sub_state_space_batch       PlannerBase::getSubStateSpace(time_steps[i]) (planner_base.h:155): sizes[i] = hm_.size()
+ *                               afterwards, 0 for a planner without a trajectory, or MPLB_ERR_STATE where the sweep met a
+ *                               successor no longer in the state space (the other entries complete; the call returns that error) */
+int mplb_lpa_get_linked_nodes_batch(mplb_planner **planners, int n, int32_t *counts, double *pts3, int64_t cap);
+int mplb_lpa_update_nodes_batch(mplb_planner **planners, int n, int blocked, const int32_t *cells3, const int64_t *offsets,
+                                int32_t *visited);
+int mplb_lpa_update_nodes_batch_device(mplb_planner **planners, int n, int blocked, const void *d_cells3, const int64_t *offsets,
+                                       int32_t *visited);
+int mplb_lpa_sub_state_space_batch(mplb_planner **planners, int n, const int32_t *time_steps, int32_t *sizes);
 /* State dumps (parity artefacts and getCloseSet / getOpenSet material): hm_ in iteration order, pq_ in its array order,
  * best_child_ (start .. goal).  Two-call pattern: cap = 0 returns the size. */
 typedef struct mplb_lpa_node {
@@ -495,6 +518,9 @@ int mplb_voxel_grid_decay(mplb_voxel_grid *g); /* decay() (vg:214-225): every ce
  * fill(nx, ny, nz) (vg:41-45); cells outside are ignored like the reference does */
 int mplb_voxel_grid_fill(mplb_voxel_grid *g, const int32_t *cells3, int n, int column);
 int mplb_voxel_grid_clear_columns(mplb_voxel_grid *g, const int32_t *cells3, int n); /* clear(nx, ny), vg:31-33, z ignored */
+/* the same two with the n cell rows in device memory, read on `stream` */
+int mplb_voxel_grid_fill_device(mplb_voxel_grid *g, const void *d_cells3, int n, int column, void *stream);
+int mplb_voxel_grid_clear_columns_device(mplb_voxel_grid *g, const void *d_cells3, int n, void *stream);
 /* getCloud (vg:18-29) / getLocalCloud (vg:47-69): centres of the cells > 0 of map_ / inflated_map_ (the local box), x outermost
  * and z innermost.  Return the number of points and write the first min(count, cap) rows of 3 doubles. */
 int64_t mplb_voxel_grid_get_cloud(mplb_voxel_grid *g, double *pts, int64_t cap);
@@ -511,6 +537,27 @@ int mplb_voxel_grid_create_map(mplb_voxel_grid *g, int inflated, mplb_map **out)
 /* MapUtil cell values for n cells (rows of 3 ints, the third ignored in 2D): the int8 value, or INT32_MIN outside the map
  * (the material of isFree / isOccupied / isUnknown, map_util.h:44-80) */
 int mplb_map_get_cells(const mplb_map *m, const int32_t *cells3, int n, int32_t *values);
+/* MapUtil::rayTrace (map_util.h:117-134) for n_rays rays, and the cell selection of the replanner node's edits
+ * (map_replanner_node.cpp:199-229), on the device.  Ray i goes from p1s[i] to p2s[i] (rows of 3 doubles; a 2D map reads the
+ * first two) and traces exactly rayTrace's cells: points n = 1 .. max_diff - 1, up to the first point outside the map, a point
+ * whose cell equals the previous point's dropped.  For every traced cell pn in trace order and every stencil offset ns[k] in
+ * the order given (n_ns rows of 3 ints, the third ignored in 2D; ns = NULL with n_ns = 0 is the single offset 0), the
+ * candidate pn + ns[k] is kept
+ *   MPLB_TRACE_ALL       always (with the offset 0 alone: rayTrace itself),
+ *   MPLB_TRACE_FREE      when it is inside the map and 0 <= value < 100 (isFree, map_util.h:44,57-62),
+ *   MPLB_TRACE_OCCUPIED  when it is inside the map and value == 100 (isOccupied, map_util.h:48,64-69),
+ * with the map's values at the call.  Duplicates from overlapping stencils stay, as in the node's new_obs list.  Returns the total
+ * count (or an error) and writes the first min(count, cap) cells as rows of 3 ints (the third 0 in 2D); offsets (may be NULL)
+ * receives n_rays + 1 entries, ray i owning rows offsets[i] .. offsets[i+1]-1.  An endpoint that is not finite, or a ray whose
+ * q / 0.8 (its longest axis in cells over 0.8) is 2^31 or more, where the reference's (int) cast is undefined, fails the call
+ * with MPLB_ERR_ARG, and so does a call with more than 2^31 - 1 candidates to examine (n_rays x max(n_ns, 1) x the points a ray
+ * can have inside the map, about 1.25 x its longest side in cells).  The _device variant takes the endpoints, cells and offsets in device memory (ns stays a host array) and
+ * orders its work on `stream`; the count is its one read-back. */
+enum { MPLB_TRACE_ALL = 0, MPLB_TRACE_FREE = 1, MPLB_TRACE_OCCUPIED = 2 };
+int64_t mplb_map_trace_cells(const mplb_map *m, const double *p1s, const double *p2s, int n_rays, const int32_t *ns, int n_ns,
+                             int select, int32_t *cells3, int64_t cap, int64_t *offsets);
+int64_t mplb_map_trace_cells_device(const mplb_map *m, const void *d_p1s, const void *d_p2s, int n_rays, const int32_t *ns, int n_ns,
+                                    int select, void *d_cells3, int64_t cap, void *d_offsets, void *stream);
 
 #ifdef __cplusplus
 }

@@ -7,6 +7,6 @@ load it, the first call does, and it raises if the library or a CUDA device is m
 """
 from . import maps  # noqa: F401
 from .planner import (ACC, ACCxYAW, JRK, JRKxYAW, SNP, SNPxYAW, VEL, VELxYAW, MapPlanner, MapUtil, MplbError, OccMapPlanner, OccMapUtil, Primitive,  # noqa: F401
-                      Trajectory, VoxelMapPlanner, VoxelMapUtil, Waypoint, waypoints_array)
+                      TRACE_ALL, TRACE_FREE, TRACE_OCCUPIED, Trajectory, VoxelMapPlanner, VoxelMapUtil, Waypoint, waypoints_array)
 from .traj_solver import TrajSolver, TrajSolver2D, TrajSolver3D  # noqa: F401,E402
 from .voxel_grid import VoxelGrid  # noqa: F401,E402

@@ -126,7 +126,17 @@ SYMBOLS = {
     "mplb_voxel_grid_write_map": (_I, [_VP, _I, _VP]),
     "mplb_voxel_grid_create_map": (_I, [_VP, _I, _VP]),
     "mplb_map_get_cells": (_I, [_VP, _VP, _I, _VP]),
+    "mplb_map_set_cells_device": (_I, [_VP, _VP, _I, _I, _VP]),
+    "mplb_voxel_grid_fill_device": (_I, [_VP, _VP, _I, _I, _VP]),
+    "mplb_voxel_grid_clear_columns_device": (_I, [_VP, _VP, _I, _VP]),
+    "mplb_map_trace_cells": (C.c_int64, [_VP, _VP, _VP, _I, _VP, _I, _I, _VP, C.c_int64, _VP]),
+    "mplb_map_trace_cells_device": (C.c_int64, [_VP, _VP, _VP, _I, _VP, _I, _I, _VP, C.c_int64, _VP, _VP]),
+    "mplb_lpa_get_linked_nodes_batch": (_I, [_VP, _I, _VP, _VP, C.c_int64]),
+    "mplb_lpa_update_nodes_batch": (_I, [_VP, _I, _I, _VP, _VP, _VP]),
+    "mplb_lpa_update_nodes_batch_device": (_I, [_VP, _I, _I, _VP, _VP, _VP]),
+    "mplb_lpa_sub_state_space_batch": (_I, [_VP, _I, _VP, _VP]),
 }
+TRACE_ALL, TRACE_FREE, TRACE_OCCUPIED = 0, 1, 2  # mplb_map_trace_cells selections
 
 PARAM = dict(v_max=0, a_max=1, j_max=2, yaw_max=3, dt=4, w=5, epsilon=6, max_num=7, tol_pos=8, tol_vel=9,
              tol_acc=10, t_max=11, potential_weight=12, gradient_weight=13, wyaw=14, mem_fraction=100, max_slots=101, exact_preds=102,

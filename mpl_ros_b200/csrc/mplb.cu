@@ -1181,6 +1181,21 @@ int mplb_map_set_cells(mplb_map *m, const int32_t *cells3, int n, int value) {
   return MPLB_OK;
 }
 
+int mplb_map_set_cells_device(mplb_map *m, const void *d_cells3, int n, int value, void *stream) {
+  if (!m || (n > 0 && !d_cells3)) return fail(MPLB_ERR_ARG, "null argument");
+  if (n <= 0) return MPLB_OK;
+  if (mplb_internal_set_device(m->device)) return fail(MPLB_ERR_CUDA, "cannot select the map's device");
+  cudaStream_t s = (cudaStream_t)stream;
+  k_set_cells<<<(n + 255) / 256, 256, 0, s>>>(m->d_grid.p, (const int *)d_cells3, n, m->dim, m->nd[0], m->nd[1], m->nd[2],
+                                             (int8_t)value);
+  g_launches++;
+  MPLB_CUDA_TRY(cudaGetLastError());
+  int rc = m->rebuild_bricks(s);
+  if (rc != MPLB_OK) return rc;
+  MPLB_CUDA_TRY(cudaStreamSynchronize(s));
+  return MPLB_OK;
+}
+
 int mplb_map_dilate(mplb_map *m, const int32_t *ns, int n) {
   if (!m || (n > 0 && !ns)) return fail(MPLB_ERR_ARG, "null argument");
   if (n <= 0) return MPLB_OK;

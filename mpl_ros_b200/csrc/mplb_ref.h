@@ -247,16 +247,20 @@ template <class M>
 MPLB_HD int cell_index(const M &m, const int *pn) { /* mu:33-41, int arithmetic like the reference (no bounds check) */
   return m.dim == 2 ? pn[0] + m.nd[0] * pn[1] : pn[0] + m.nd[0] * pn[1] + m.nd[0] * m.nd[1] * pn[2];
 }
-/* rayTrace (mu:117-134) from p1 to p2: returns max_diff (points n = 1 .. max_diff - 1 are traced), writes diff = p2 - p1
- * and s = 1 / max_diff.  The reference takes std::max over the axes starting from 0; fmax is the same for these non-negative
- * values and also skips a NaN. */
-MPLB_HD int ray_setup(int dim, double res, const double *p1, const double *p2, double *diff, double *s) {
+/* rayTrace (mu:117-134) from p1 to p2: ray_span writes diff = p2 - p1 and returns q / 0.8 (q = the largest |diff| / res over
+ * the axes); ray_setup returns max_diff = (int)(q / 0.8) (points n = 1 .. max_diff - 1 are traced) and writes s = 1 / max_diff.
+ * The reference takes std::max over the axes starting from 0; fmax is the same for these non-negative values and also skips a
+ * NaN.  The cast is undefined unless q / 0.8 < 2^31, which a caller taking endpoints from outside checks with ray_span. */
+MPLB_HD double ray_span(int dim, double res, const double *p1, const double *p2, double *diff) {
   double q = 0;
   for (int i = 0; i < dim; i++) {
     diff[i] = dsub(p2[i], p1[i]);
     q = fmax(q, fabs(ddiv(diff[i], res)));
   }
-  const int max_diff = (int)ddiv(q, 0.8);
+  return ddiv(q, 0.8);
+}
+MPLB_HD int ray_setup(int dim, double res, const double *p1, const double *p2, double *diff, double *s) {
+  const int max_diff = (int)ray_span(dim, res, p1, p2, diff);
   *s = ddiv(1.0, (double)max_diff);
   return max_diff;
 }

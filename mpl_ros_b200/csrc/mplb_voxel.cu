@@ -201,6 +201,116 @@ __global__ void k_map_get_cells(const int8_t *grid, int dim, int nx, int ny, int
                                                                           : (int)grid[(size_t)x + (size_t)nx * y + (size_t)nx * ny * z];
 }
 
+/* ---- MapUtil::rayTrace (mu:117-134) and the replanner node's cell selection (map_replanner_node.cpp:199-219,221-229).
+ * Ray r examines its points n = 1 .. len[r] (slot r * B + n - 1; B bounds the points a ray can have inside the map), cut[r] is
+ * its first point outside the map (or len[r] + 1), and a point is traced when it comes before the cut and its cell differs
+ * from the previous point's. */
+__device__ __forceinline__ void ray_ends(const MplbMapView &m, const double *p1s, const double *p2s, long long r, double *a, double *b) {
+  for (int k = 0; k < m.dim; k++) { a[k] = p1s[r * 3 + k]; b[k] = p2s[r * 3 + k]; }
+}
+__device__ __forceinline__ void ray_cell(const MplbMapView &m, const double *a, const double *diff, double s, int n, int *pn) {
+  double pt[3];
+  for (int k = 0; k < m.dim; k++) pt[k] = ray_point(a[k], diff[k], s, n);
+  float_to_int(m, pt, pn);
+}
+__device__ __forceinline__ bool trace_keep(const MplbMapView &m, const int *c, int select) {
+  if (select == MPLB_TRACE_ALL) return true;
+  if (outside(m, c)) return false; /* isFree / isOccupied are false outside (mu:44-69) */
+  const int8_t v = m.d_grid[(size_t)c[0] + (size_t)m.nd[0] * c[1] + (m.dim == 3 ? (size_t)m.nd[0] * m.nd[1] * c[2] : 0)];
+  return select == MPLB_TRACE_FREE ? (v >= 0 && v < 100) : v == 100;
+}
+
+/* one thread per ray: the endpoint checks, the points to examine, the initial cut */
+__global__ void k_trace_rays(MplbMapView m, const double *p1s, const double *p2s, int n_rays, int B, int *len, int *cut, int *bad) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n_rays) return;
+  double a[3], b[3], diff[3];
+  ray_ends(m, p1s, p2s, r, a, b);
+  bool ok = true;
+  for (int k = 0; k < m.dim; k++) ok = ok && isfinite(a[k]) && isfinite(b[k]);
+  ok = ok && ray_span(m.dim, m.res, a, b, diff) < 2147483648.0;
+  int l = 0;
+  if (ok) {
+    double s;
+    l = min(ray_setup(m.dim, m.res, a, b, diff, &s) - 1, B);
+    if (l < 0) l = 0;
+  } else {
+    atomicOr(bad, 1);
+  }
+  len[r] = l;
+  cut[r] = l + 1;
+}
+/* one thread per slot: the first point outside the map cuts the ray */
+__global__ void k_trace_cut(MplbMapView m, const double *p1s, const double *p2s, long long slots, int B, const int *len, int *cut) {
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < slots; t += (long long)gridDim.x * blockDim.x) {
+    const long long r = t / B;
+    const int n = (int)(t % B) + 1;
+    if (n > len[r]) continue;
+    double a[3], b[3], diff[3], s;
+    ray_ends(m, p1s, p2s, r, a, b);
+    ray_setup(m.dim, m.res, a, b, diff, &s);
+    int pn[3];
+    ray_cell(m, a, diff, s, n, pn);
+    if (outside(m, pn)) atomicMin(&cut[r], n);
+  }
+}
+/* slot t's traced cell (false when the slot traces none) */
+__device__ __forceinline__ bool slot_cell(const MplbMapView &m, const double *p1s, const double *p2s, long long t, int B, const int *cut,
+                                          int *pn) {
+  const long long r = t / B;
+  const int n = (int)(t % B) + 1;
+  if (n >= cut[r]) return false;
+  double a[3], b[3], diff[3], s;
+  ray_ends(m, p1s, p2s, r, a, b);
+  ray_setup(m.dim, m.res, a, b, diff, &s);
+  ray_cell(m, a, diff, s, n, pn);
+  if (n == 1) return true; /* the reference's previous cell starts at -1, never a cell inside */
+  int pp[3];
+  ray_cell(m, a, diff, s, n - 1, pp);
+  return pn[0] != pp[0] || pn[1] != pp[1] || pn[2] != pp[2];
+}
+/* one thread per slot: how many of its candidates pn + ns[k] the selection keeps */
+__global__ void k_trace_count(MplbMapView m, const double *p1s, const double *p2s, long long slots, int B, const int *cut, const int *ns,
+                              int n_ns, int select, int *cnt) {
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < slots; t += (long long)gridDim.x * blockDim.x) {
+    int pn[3];
+    int c = 0;
+    if (slot_cell(m, p1s, p2s, t, B, cut, pn))
+      for (int k = 0; k < n_ns; k++) {
+        const int q[3] = {pn[0] + ns[k * 3], pn[1] + ns[k * 3 + 1], m.dim == 3 ? pn[2] + ns[k * 3 + 2] : 0};
+        c += trace_keep(m, q, select);
+      }
+    cnt[t] = c;
+  }
+}
+/* one thread per slot: its kept candidates at their place in (ray, point, offset) order (pos = exclusive scan of the counts),
+ * the first `cap` rows only; offsets[r] and, from slot 0, offsets[n_rays] and the total (-1: an endpoint was rejected) */
+__global__ void k_trace_emit(MplbMapView m, const double *p1s, const double *p2s, int n_rays, long long slots, int B, const int *cut,
+                             const int *ns, int n_ns, int select, const int *cnt, const int *pos, const int *bad, int *out, long long cap,
+                             long long *offsets, long long *total) {
+  if (*bad) {
+    if (blockIdx.x == 0 && threadIdx.x == 0) *total = -1;
+    return;
+  }
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < slots; t += (long long)gridDim.x * blockDim.x) {
+    long long w = pos[t];
+    if (offsets && t % B == 0) offsets[t / B] = w;
+    if (t == 0) {
+      const long long all = (long long)pos[slots - 1] + cnt[slots - 1];
+      if (offsets) offsets[n_rays] = all;
+      *total = all;
+    }
+    int pn[3];
+    if (w >= cap || !slot_cell(m, p1s, p2s, t, B, cut, pn)) continue;
+    for (int k = 0; k < n_ns && w < cap; k++) {
+      const int q[3] = {pn[0] + ns[k * 3], pn[1] + ns[k * 3 + 1], m.dim == 3 ? pn[2] + ns[k * 3 + 2] : 0};
+      if (!trace_keep(m, q, select)) continue;
+      out[w * 3] = q[0]; out[w * 3 + 1] = q[1]; out[w * 3 + 2] = q[2];
+      w++;
+    }
+  }
+}
+
 int key_bits(unsigned ncell) { /* radix-sort bits covering keys 0 .. ncell */
   int b = 1;
   while (b < 32 && (1ull << b) <= ncell) b++;
@@ -386,17 +496,101 @@ int upload_cells(mplb_voxel_grid *g, const int32_t *cells3, int n) {
   return MPLB_OK;
 }
 
-int vg_edit(mplb_voxel_grid *g, const int32_t *cells3, int n, int column, int8_t value) {
+/* fill / clear with the cell rows on the host (device = false) or already on the grid's device, read on `stream` */
+int vg_edit(mplb_voxel_grid *g, const int32_t *cells3, int n, int column, int8_t value, bool device, cudaStream_t stream) {
   int rc = check_grid(g);
   if (rc) return rc;
   if (n < 0 || (n > 0 && !cells3)) return mplb_internal_fail(MPLB_ERR_ARG, "bad cell buffer");
   if (n == 0 || !g->ncell) return MPLB_OK;
-  rc = upload_cells(g, cells3, n);
-  if (rc) return rc;
-  k_vg_fill<<<(n + 255) / 256, 256>>>(g->d_map.p, g->cells.p, n, column, value, g->dim[0], g->dim[1], g->dim[2]);
+  const int *d_cells = (const int *)cells3;
+  if (!device) {
+    rc = upload_cells(g, cells3, n);
+    if (rc) return rc;
+    d_cells = g->cells.p;
+  }
+  k_vg_fill<<<(n + 255) / 256, 256, 0, stream>>>(g->d_map.p, d_cells, n, column, value, g->dim[0], g->dim[1], g->dim[2]);
   mplb_internal_count_launches(1);
   MPLB_CUDA_TRY(cudaGetLastError());
-  MPLB_CUDA_TRY(cudaDeviceSynchronize());
+  MPLB_CUDA_TRY(device ? cudaStreamSynchronize(stream) : cudaDeviceSynchronize());
+  return MPLB_OK;
+}
+
+/* scratch of the ray tracer, per host thread (re-created when the thread's current device changes) */
+struct TraceScratch {
+  int device = -1;
+  DevBuf<int> len, cut, ns, bad, out, cnt, pos;
+  DevBuf<long long> total, offs;
+  DevBuf<double> pts;
+  DevBuf<char> tmp;
+};
+thread_local TraceScratch g_trace;
+TraceScratch &trace_scratch(int device) {
+  if (g_trace.device != device) { g_trace = TraceScratch(); g_trace.device = device; }
+  return g_trace;
+}
+
+/* rays examine up to B points each: consecutive points are at least 0.8 res apart on the ray's dominant axis, so no ray has
+ * more points inside the map before its first one outside */
+int trace_points_per_ray(const MplbMapView &v) {
+  int max_nd = 0;
+  for (int k = 0; k < v.dim; k++) max_nd = std::max(max_nd, v.nd[k]);
+  return (int)((max_nd + 2.0) / 0.8) + 2;
+}
+/* the most rows a call can select */
+int64_t trace_bound(const MplbMapView &v, int n_rays, int n_ns) {
+  return (int64_t)n_rays * trace_points_per_ray(v) * std::max(n_ns, 1);
+}
+
+/* rays (d_p1s, d_p2s: device rows of 3 doubles) through map view v on stream st: the first `cap` selected cells to d_out, the
+ * n_rays + 1 offsets to d_offsets (may be NULL); returns the total count or an error */
+int64_t trace_cells(const MplbMapView &v, const double *d_p1s, const double *d_p2s, int n_rays, const int32_t *ns, int n_ns,
+                    int select, int *d_out, int64_t cap, long long *d_offsets, cudaStream_t st) {
+  TraceScratch &g = trace_scratch(v.device);
+  if (n_rays == 0) {
+    if (d_offsets) MPLB_CUDA_TRY(cudaMemsetAsync(d_offsets, 0, sizeof(long long), st));
+    MPLB_CUDA_TRY(cudaStreamSynchronize(st));
+    return 0;
+  }
+  const int zero3[3] = {0, 0, 0};
+  if (n_ns == 0) { ns = zero3; n_ns = 1; } /* the offset 0 alone: the ray's own cells */
+  const int B = trace_points_per_ray(v);
+  const long long slots = (long long)n_rays * B;
+  if (slots * n_ns > 0x7fffffff) return mplb_internal_fail(MPLB_ERR_ARG, "trace_cells: more than 2^31 - 1 candidate cells to examine");
+  MPLB_CUDA_TRY(g.len.reserve(n_rays));
+  MPLB_CUDA_TRY(g.cut.reserve(n_rays));
+  MPLB_CUDA_TRY(g.bad.reserve(1));
+  MPLB_CUDA_TRY(g.total.reserve(1));
+  MPLB_CUDA_TRY(g.ns.reserve((size_t)n_ns * 3));
+  MPLB_CUDA_TRY(g.cnt.reserve(slots));
+  MPLB_CUDA_TRY(g.pos.reserve(slots));
+  MPLB_CUDA_TRY(cudaMemcpyAsync(g.ns.p, ns, (size_t)n_ns * 3 * sizeof(int), cudaMemcpyHostToDevice, st));
+  MPLB_CUDA_TRY(cudaMemsetAsync(g.bad.p, 0, sizeof(int), st));
+  size_t tmp_bytes = 0;
+  MPLB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, g.cnt.p, g.pos.p, (int)slots, st));
+  MPLB_CUDA_TRY(g.tmp.reserve(std::max<size_t>(tmp_bytes, 1)));
+  k_trace_rays<<<(n_rays + 127) / 128, 128, 0, st>>>(v, d_p1s, d_p2s, n_rays, B, g.len.p, g.cut.p, g.bad.p);
+  k_trace_cut<<<blocks_for((size_t)slots), 256, 0, st>>>(v, d_p1s, d_p2s, slots, B, g.len.p, g.cut.p);
+  k_trace_count<<<blocks_for((size_t)slots), 256, 0, st>>>(v, d_p1s, d_p2s, slots, B, g.cut.p, g.ns.p, n_ns, select, g.cnt.p);
+  MPLB_CUDA_TRY(cudaGetLastError());
+  MPLB_CUDA_TRY(cub::DeviceScan::ExclusiveSum(g.tmp.p, tmp_bytes, g.cnt.p, g.pos.p, (int)slots, st));
+  k_trace_emit<<<blocks_for((size_t)slots), 256, 0, st>>>(v, d_p1s, d_p2s, n_rays, slots, B, g.cut.p, g.ns.p, n_ns, select, g.cnt.p,
+                                                           g.pos.p, g.bad.p, d_out, cap, d_offsets, g.total.p);
+  mplb_internal_count_launches(5);
+  MPLB_CUDA_TRY(cudaGetLastError());
+  long long total = 0;
+  MPLB_CUDA_TRY(cudaMemcpyAsync(&total, g.total.p, sizeof(total), cudaMemcpyDeviceToHost, st));
+  MPLB_CUDA_TRY(cudaStreamSynchronize(st));
+  if (total < 0) return mplb_internal_fail(MPLB_ERR_ARG, "trace_cells: an endpoint is not finite, or a ray has 2^31 or more steps");
+  return total;
+}
+
+int check_trace_args(const mplb_map *m, int n_rays, bool rays, const int32_t *ns, int n_ns, int select, bool out, int64_t cap) {
+  if (!m) return mplb_internal_fail(MPLB_ERR_ARG, "null map");
+  if (n_rays < 0 || (n_rays > 0 && !rays)) return mplb_internal_fail(MPLB_ERR_ARG, "bad ray buffers");
+  if (n_ns < 0 || (n_ns > 0 && !ns)) return mplb_internal_fail(MPLB_ERR_ARG, "bad stencil");
+  if (select != MPLB_TRACE_ALL && select != MPLB_TRACE_FREE && select != MPLB_TRACE_OCCUPIED)
+    return mplb_internal_fail(MPLB_ERR_ARG, "unknown selection");
+  if (cap < 0 || (cap > 0 && !out)) return mplb_internal_fail(MPLB_ERR_ARG, "bad output buffer");
   return MPLB_OK;
 }
 
@@ -521,10 +715,18 @@ int mplb_voxel_grid_decay(mplb_voxel_grid *g) {
 }
 
 int mplb_voxel_grid_fill(mplb_voxel_grid *g, const int32_t *cells3, int n, int column) {
-  return vg_edit(g, cells3, n, column ? 1 : 0, 100);
+  return vg_edit(g, cells3, n, column ? 1 : 0, 100, false, nullptr);
 }
 
-int mplb_voxel_grid_clear_columns(mplb_voxel_grid *g, const int32_t *cells3, int n) { return vg_edit(g, cells3, n, 1, 0); }
+int mplb_voxel_grid_clear_columns(mplb_voxel_grid *g, const int32_t *cells3, int n) { return vg_edit(g, cells3, n, 1, 0, false, nullptr); }
+
+int mplb_voxel_grid_fill_device(mplb_voxel_grid *g, const void *d_cells3, int n, int column, void *stream) {
+  return vg_edit(g, (const int32_t *)d_cells3, n, column ? 1 : 0, 100, true, (cudaStream_t)stream);
+}
+
+int mplb_voxel_grid_clear_columns_device(mplb_voxel_grid *g, const void *d_cells3, int n, void *stream) {
+  return vg_edit(g, (const int32_t *)d_cells3, n, 1, 0, true, (cudaStream_t)stream);
+}
 
 int64_t mplb_voxel_grid_get_cloud(mplb_voxel_grid *g, double *pts, int64_t cap) {
   int rc = check_grid(g);
@@ -610,6 +812,42 @@ int mplb_map_get_cells(const mplb_map *m, const int32_t *cells3, int n, int32_t 
   MPLB_CUDA_TRY(cudaGetLastError());
   MPLB_CUDA_TRY(cudaMemcpy(values, d.p + (size_t)n * 3, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost));
   return MPLB_OK;
+}
+
+int64_t mplb_map_trace_cells(const mplb_map *m, const double *p1s, const double *p2s, int n_rays, const int32_t *ns, int n_ns,
+                             int select, int32_t *cells3, int64_t cap, int64_t *offsets) {
+  int rc = check_trace_args(m, n_rays, p1s && p2s, ns, n_ns, select, cells3 != nullptr, cap);
+  if (rc) return rc;
+  MplbMapView v;
+  mplb_internal_map_view(const_cast<mplb_map *>(m), &v);
+  if (mplb_internal_set_device(v.device)) return mplb_internal_fail(MPLB_ERR_CUDA, "cannot select the map's device");
+  TraceScratch &g = trace_scratch(v.device);
+  const int64_t rows = std::min<int64_t>(cap, trace_bound(v, n_rays, n_ns));
+  MPLB_CUDA_TRY(g.pts.reserve((size_t)std::max(n_rays, 1) * 6));
+  MPLB_CUDA_TRY(g.out.reserve((size_t)std::max<int64_t>(rows, 1) * 3));
+  MPLB_CUDA_TRY(g.offs.reserve((size_t)n_rays + 1));
+  if (n_rays > 0) {
+    MPLB_CUDA_TRY(cudaMemcpy(g.pts.p, p1s, (size_t)n_rays * 3 * sizeof(double), cudaMemcpyHostToDevice));
+    MPLB_CUDA_TRY(cudaMemcpy(g.pts.p + (size_t)n_rays * 3, p2s, (size_t)n_rays * 3 * sizeof(double), cudaMemcpyHostToDevice));
+  }
+  const int64_t total = trace_cells(v, g.pts.p, g.pts.p + (size_t)n_rays * 3, n_rays, ns, n_ns, select, g.out.p, rows, g.offs.p, 0);
+  if (total < 0) return total;
+  if (offsets) MPLB_CUDA_TRY(cudaMemcpy(offsets, g.offs.p, ((size_t)n_rays + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost));
+  const int64_t got = std::min<int64_t>(total, rows);
+  if (got > 0) MPLB_CUDA_TRY(cudaMemcpy(cells3, g.out.p, (size_t)got * 3 * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  return total;
+}
+
+int64_t mplb_map_trace_cells_device(const mplb_map *m, const void *d_p1s, const void *d_p2s, int n_rays, const int32_t *ns, int n_ns,
+                                    int select, void *d_cells3, int64_t cap, void *d_offsets, void *stream) {
+  int rc = check_trace_args(m, n_rays, d_p1s && d_p2s, ns, n_ns, select, d_cells3 != nullptr, cap);
+  if (rc) return rc;
+  MplbMapView v;
+  mplb_internal_map_view(const_cast<mplb_map *>(m), &v);
+  if (mplb_internal_set_device(v.device)) return mplb_internal_fail(MPLB_ERR_CUDA, "cannot select the map's device");
+  trace_scratch(v.device);
+  return trace_cells(v, (const double *)d_p1s, (const double *)d_p2s, n_rays, ns, n_ns, select, (int *)d_cells3, cap,
+                     (long long *)d_offsets, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -19,6 +19,7 @@ from .maps import ACC, JRK, SNP, VEL  # noqa: F401
 
 VELxYAW, ACCxYAW, JRKxYAW, SNPxYAW = VEL | 16, ACC | 16, JRK | 16, SNP | 16  # control.h:15-18
 
+TRACE_ALL, TRACE_FREE, TRACE_OCCUPIED = _lib.TRACE_ALL, _lib.TRACE_FREE, _lib.TRACE_OCCUPIED  # MapUtil.traceCells selections
 PLAN_OK, PLAN_START_NOT_FREE, PLAN_MAX_EXPAND, PLAN_QUEUE_EMPTY, PLAN_TRACEBACK_FAILED, PLAN_START_IS_GOAL = range(6)
 
 
@@ -180,6 +181,37 @@ class MapUtil:
         out = np.zeros(max(len(c3), 1), dtype=np.int32)
         check(lib().mplb_map_get_cells(self._h, ptr(c3), len(c3), ptr(out)))
         return out[:len(c3)]
+
+    def traceCells(self, p1s, p2s, ns=None, select=_lib.TRACE_ALL):
+        """rayTrace (map_util.h:117-134) of every ray p1s[i] -> p2s[i] on the GPU, then the cells pn + ns[k] of every traced
+        cell pn and stencil offset (ns rows of Dim ints; None is the offset 0) that `select` keeps: TRACE_ALL all of them,
+        TRACE_FREE the isFree ones, TRACE_OCCUPIED the isOccupied ones (mplb_map_trace_cells).  Returns (cells (k, Dim) int32,
+        offsets (n_rays + 1) int64): ray i owns cells[offsets[i]:offsets[i + 1]]."""
+        a, b = self._rows3(p1s, np.float64), self._rows3(p2s, np.float64)
+        if len(a) != len(b):
+            raise MplbError("p1s and p2s differ in length")
+        ns3 = None if ns is None else self._rows3(ns, np.int32)
+        n_ns = 0 if ns3 is None else len(ns3)
+        offs = np.zeros(len(a) + 1, dtype=np.int64)
+        cap = 4096
+        while True:
+            out = np.zeros((cap, 3), dtype=np.int32)
+            k = check(lib().mplb_map_trace_cells(self._h, ptr(a), ptr(b), len(a), ptr(ns3) if n_ns else None, n_ns, int(select),
+                                                 ptr(out), cap, ptr(offs)))
+            if k <= cap:
+                return out[:k, :self.dim].copy(), offs
+            cap = k
+
+    def rayTrace(self, pt1, pt2):  # map_util.h:117-134
+        return self.traceCells([pt1], [pt2])[0]
+
+    @staticmethod
+    def _rows3(rows, dtype):
+        r = np.asarray(rows, dtype=dtype)
+        r = r.reshape(len(r), -1) if r.size else r.reshape(len(r), 0)
+        out = np.zeros((len(r), 3), dtype=dtype)
+        out[:, :r.shape[1]] = r
+        return out
 
     def freeUnknown(self):  # map_util.h:259-276
         check(lib().mplb_map_free_unknown(self._h))
@@ -427,11 +459,16 @@ class MapPlanner:
             goal.to_record(g[0])
         res = np.zeros(1, dtype=_lib.RESULT_DTYPE)
         check(lib().mplb_plan(self._h, ptr(s), ptr(g), ptr(res)))
-        self._last = res[0]
-        self._control = int(s["control"][0])
+        return self._planned(res[0], int(s["control"][0]))
+
+    def _planned(self, res, control):
+        """plan()'s bookkeeping after the library planned: result record, traj_cost_ and traj_"""
+        res = np.array(res, dtype=_lib.RESULT_DTYPE)[()]
+        self._last = res
+        self._control = control
         self._initialized = True
-        self.traj_cost_ = float(res[0]["cost"])
-        st = int(res[0]["status"])
+        self.traj_cost_ = float(res["cost"])
+        st = int(res["status"])
         # traj_ is rewritten only where the reference writes it: recoverTraj success or failure (graph_search.h:447-451).
         # start-not-free (planner_base.h:283-287), start-is-goal (graph_search.h:44), MaxExpandStep and empty queue
         # (graph_search.h:149-161) leave the previous trajectory in place.
@@ -468,6 +505,71 @@ class MapPlanner:
     def updateClearedNodes(self, cleared_pns):  # map_planner.cpp:173-185
         c3 = self._cells3(cleared_pns)
         return check(lib().mplb_update_cleared_nodes(self._h, ptr(c3), len(c3)))
+
+    # ---- fleets: one call per replan step for many planners (each entry leaves its planner as the single call would)
+    @staticmethod
+    def _handles(planners):
+        return (C.c_void_p * max(len(planners), 1))(*[p._h for p in planners])
+
+    @staticmethod
+    def planLPABatch(planners, starts, goals):
+        """mplb_lpa_plan_batch: planner i plans starts[i] -> goals[i] (Waypoint objects or waypoint records) in one launch per
+        session kind, and keeps result(), traj_, traj_cost_ exactly as plan() would.  Returns plan()'s booleans."""
+        n = len(planners)
+        s, g = waypoints_array(n), waypoints_array(n)
+        for i in range(n):
+            for src, dst in ((starts[i], s), (goals[i], g)):
+                if isinstance(src, Waypoint):
+                    src.to_record(dst[i])
+                else:
+                    dst[i] = np.asarray(src).reshape(-1)[0] if np.ndim(src) else src
+        res = np.zeros(max(n, 1), dtype=_lib.RESULT_DTYPE)
+        check(lib().mplb_lpa_plan_batch(MapPlanner._handles(planners), n, ptr(s), ptr(g), ptr(res)))
+        return [pl._planned(res[i], int(s["control"][i])) for i, pl in enumerate(planners)]
+
+    @staticmethod
+    def getLinkedNodesBatch(planners):
+        """getLinkedNodes of every planner (mplb_lpa_get_linked_nodes_batch): a list of (k_i, Dim) point arrays"""
+        n = len(planners)
+        h = MapPlanner._handles(planners)
+        counts = np.zeros(max(n, 1), dtype=np.int32)
+        check(lib().mplb_lpa_get_linked_nodes_batch(h, n, ptr(counts), None, 0))
+        total = int(counts[:n].sum())
+        pts = np.zeros((max(total, 1), 3), dtype=np.float64)
+        check(lib().mplb_lpa_get_linked_nodes_batch(h, n, ptr(counts), ptr(pts), total))
+        off = np.concatenate([[0], np.cumsum(counts[:n])])
+        return [pts[off[i]:off[i + 1], :pl.dim].copy() for i, pl in enumerate(planners)]
+
+    @staticmethod
+    def _update_batch(planners, cell_lists, blocked):
+        n = len(planners)
+        c3 = [planners[i]._cells3(c) if len(c) else np.zeros((0, 3), dtype=np.int32) for i, c in enumerate(cell_lists)]
+        offs = np.zeros(n + 1, dtype=np.int64)
+        offs[1:] = np.cumsum([len(c) for c in c3])
+        cells = np.ascontiguousarray(np.concatenate(c3) if n else np.zeros((0, 3)), dtype=np.int32)
+        visited = np.zeros(max(n, 1), dtype=np.int32)
+        check(lib().mplb_lpa_update_nodes_batch(MapPlanner._handles(planners), n, int(blocked), ptr(cells) if len(cells) else None,
+                                                ptr(offs), ptr(visited)))
+        return [int(v) for v in visited[:n]]
+
+    @staticmethod
+    def updateBlockedNodesBatch(planners, cell_lists):
+        """updateBlockedNodes(cell_lists[i]) on planner i (mplb_lpa_update_nodes_batch); returns the visited pair counts"""
+        return MapPlanner._update_batch(planners, cell_lists, True)
+
+    @staticmethod
+    def updateClearedNodesBatch(planners, cell_lists):
+        """updateClearedNodes(cell_lists[i]) on planner i; returns the visited pair counts"""
+        return MapPlanner._update_batch(planners, cell_lists, False)
+
+    @staticmethod
+    def getSubStateSpaceBatch(planners, time_steps):
+        """getSubStateSpace(time_steps[i]) on planner i (mplb_lpa_sub_state_space_batch); returns the hm_ sizes"""
+        n = len(planners)
+        ts = np.ascontiguousarray(time_steps, dtype=np.int32).reshape(n) if n else np.zeros(1, dtype=np.int32)
+        sizes = np.zeros(max(n, 1), dtype=np.int32)
+        check(lib().mplb_lpa_sub_state_space_batch(MapPlanner._handles(planners), n, ptr(ts), ptr(sizes)))
+        return [int(v) for v in sizes[:n]]
 
     def lpaNodes(self):
         """hm_ in iteration order (state dump: key, coord, g, rhs, h, flags, list hashes)"""
