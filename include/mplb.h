@@ -180,7 +180,8 @@ int mplb_planner_set_controls(mplb_planner *p, const double *U, int n, int udim)
 
 /* ---- cost shaping of env_map (SURVEY section 8f.1): search region and potential map, env_map.h:104-128.
  * Both are per-planner state like ENV_->search_region_ / potential_map_ and stay set until replaced or cleared.
- * Shaped plans need |U| <= 32 and a map that was scrubbed of unknown cells or not (either works). */
+ * Shaped plans take control sets of up to 128 rows (|U| > 32 runs on the shaped MAXU = 4 kernels) and need positive dynamic
+ * bounds for every derivative of the control order; the map may be scrubbed of unknown cells or not (either works). */
 /* env_base::set_search_region (env_base.h:301-303): one byte (0/1) per map cell, x fastest.  NULL or n = 0 clears. */
 int mplb_planner_set_search_region(mplb_planner *p, const uint8_t *in_region, size_t n);
 /* MapPlanner::setSearchRegion (map_planner.cpp:46-95): tunnel of half-width `radius` (Dim doubles, setSearchRadius

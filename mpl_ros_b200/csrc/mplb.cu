@@ -326,7 +326,9 @@ struct mplb_planner {
   int max_num = -1;
   double mem_fraction = 0.6;
   int max_slots = 0; /* 0 = as many CTAs as are resident */
-  int resident_sig = -1, resident_cached = 0, hcap_big_cached = 0, sm_count = 0;
+  long long resident_sig = -1;
+  int resident_cached = 0, hcap_small_cached = 0, hcap_big_cached = 0, sm_count = 0;
+  size_t term_bytes = 0; /* |U| > 32 cost-shaping plans: per-sample term pairs behind the heap top (PlanSmem::DYN_TERMS) */
   size_t budget_bytes = 0; /* arena budget, measured at the first batch (reset by MPLB_MEM_FRACTION / MPLB_ARENA_BYTES) */
   size_t arena_bytes = 0;  /* MPLB_ARENA_BYTES: upper bound on the budget, 0 = unset */
   int lpa_init_nodes = 1 << 16, lpa_init_preds = 1 << 20; /* MPLB_LPA_INIT_NODES / _PREDS: LPA* array sizes at allocation */
@@ -563,10 +565,16 @@ int build_cfg(mplb_planner *p, int control) {
   if (shaped) {
     if (p->pot_cells && p->pot_cells != m->ncell) return fail(MPLB_ERR_STATE, "potential map size does not match the planner's map");
     if (!p->h_region.empty() && p->h_region.size() != m->ncell) return fail(MPLB_ERR_STATE, "search region size does not match the planner's map");
-    if (p->nU > 32) return fail(MPLB_ERR_ARG, "search region / potential map / yaw controls need a control set of at most 32 rows");
     if (!c.use_fast) return fail(MPLB_ERR_ARG, "search region / potential map / yaw controls need positive dynamic bounds for every derivative of the control order");
     if (p->pot_cells) c.pot = p->d_pot.p;
     if (!p->h_region.empty()) c.region = p->d_region.p;
+  }
+  /* a |U| > 32 cost-shaping launch keeps every sample term of one expansion in shared memory: 8 slots per granule, as many
+   * granules per control as the longest sample list (tcnt[n] <= n + 1) needs */
+  p->term_bytes = 0;
+  if (shaped && p->nU > 32) {
+    const int cnt_hi = *std::max_element(tcnt.begin(), tcnt.end());
+    p->term_bytes = (size_t)p->nU * 8 * ((cnt_hi + 7) / 8) * (2 * sizeof(double));
   }
   /* prior trajectory (eb:46-53, em:187-225 without a potential map) */
   c.prior = nullptr; c.prior_n = 0; c.prior_on = 0;
@@ -692,16 +700,17 @@ int build_cfg(mplb_planner *p, int control) {
   return MPLB_OK;
 }
 
-/* shared memory of one CTA: the plan record, plus (|U| > 32 instantiations) `hcap` heap entries of 20 bytes behind it */
+/* shared memory of one CTA: the plan record, plus (|U| > 32 instantiations) `hcap` heap entries of 20 bytes behind it,
+ * plus (|U| > 32 cost-shaping instantiations) the launch's `term_bytes` of sample terms behind those */
 template <int DIM, int ORD, int MAXU, bool POT>
-size_t smem_bytes(int hcap) {
+size_t smem_bytes(int hcap, size_t term_bytes) {
   using SM = PlanSmem<DIM, ORD, MAXU, POT>;
-  return SM::DYN_HEAP ? heap_dyn_offset<SM>() + (size_t)hcap * 20 : sizeof(SM);
+  return SM::DYN_HEAP ? heap_dyn_offset<SM>() + (size_t)hcap * 20 + (SM::DYN_TERMS ? term_bytes : 0) : sizeof(SM);
 }
 
 template <int DIM, int ORD, int MAXU, bool POT>
-int launch_batch(const DevCfg &c, const BatchArgs &a, int grid, cudaStream_t s) {
-  size_t smem = smem_bytes<DIM, ORD, MAXU, POT>(a.hcap);
+int launch_batch(const DevCfg &c, const BatchArgs &a, size_t term_bytes, int grid, cudaStream_t s) {
+  size_t smem = smem_bytes<DIM, ORD, MAXU, POT>(a.hcap, term_bytes);
   auto kern = astar_batch_kernel<DIM, ORD, MAXU, POT>;
   if (smem > 48 * 1024) MPLB_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared); /* residency is shared-memory bound */
@@ -739,9 +748,9 @@ int launch_batch(const DevCfg &c, const BatchArgs &a, int grid, cudaStream_t s) 
 }
 
 template <int DIM, int ORD, int MAXU, bool POT>
-int resident_ctas(int device, int hcap) {
+int resident_ctas(int device, int hcap, size_t term_bytes) {
   int per_sm = 0, sms = 0;
-  size_t smem = smem_bytes<DIM, ORD, MAXU, POT>(hcap);
+  size_t smem = smem_bytes<DIM, ORD, MAXU, POT>(hcap, term_bytes);
   auto kern = astar_batch_kernel<DIM, ORD, MAXU, POT>;
   if (smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
@@ -750,25 +759,30 @@ int resident_ctas(int device, int hcap) {
   return per_sm * sms;
 }
 
-/* the cost-shaping kernels exist for |U| <= 32 only (build_cfg rejects larger control sets with shaping) */
 template <int DIM, int ORD, int MAXU>
-int launch_any(bool shaped, const DevCfg &c, const BatchArgs &a, int grid, cudaStream_t s) {
-  if constexpr (MAXU == 1) { if (shaped) return launch_batch<DIM, ORD, MAXU, true>(c, a, grid, s); }
-  return launch_batch<DIM, ORD, MAXU, false>(c, a, grid, s);
+int launch_any(bool shaped, const DevCfg &c, const BatchArgs &a, size_t term_bytes, int grid, cudaStream_t s) {
+  if (shaped) return launch_batch<DIM, ORD, MAXU, true>(c, a, term_bytes, grid, s);
+  return launch_batch<DIM, ORD, MAXU, false>(c, a, term_bytes, grid, s);
 }
 template <int DIM, int ORD, int MAXU>
-int resident_any(bool shaped, int device, int hcap) {
-  if constexpr (MAXU == 1) { if (shaped) return resident_ctas<DIM, ORD, MAXU, true>(device, hcap); }
-  return resident_ctas<DIM, ORD, MAXU, false>(device, hcap);
+int resident_any(bool shaped, int device, int hcap, size_t term_bytes) {
+  if (shaped) return resident_ctas<DIM, ORD, MAXU, true>(device, hcap, term_bytes);
+  return resident_ctas<DIM, ORD, MAXU, false>(device, hcap, term_bytes);
 }
-/* largest shared-memory heap of a |U| > 32 launch that runs one plan per SM */
-template <int DIM, int ORD, int MAXU>
-int hcap_big(int device) {
+/* heap entries of a |U| > 32 launch that fit in one CTA's shared memory next to the plan record and, in the cost-shaping
+ * instantiations, the term area: a multiple of 256, at most 8192 */
+template <int DIM, int ORD, int MAXU, bool POT>
+int hcap_room(int device, size_t term_bytes) {
   int optin = 0;
   if (cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device) != cudaSuccess) return MPLB_HCAP_SMALL;
-  const long long room = (long long)optin - (long long)heap_dyn_offset<PlanSmem<DIM, ORD, MAXU, false>>() - 1024;
-  long long h = room / 20 / 256 * 256;
-  return (int)std::max<long long>(MPLB_HCAP_SMALL, std::min<long long>(h, 8192));
+  const long long room = (long long)optin - (long long)heap_dyn_offset<PlanSmem<DIM, ORD, MAXU, POT>>() -
+                         (PlanSmem<DIM, ORD, MAXU, POT>::DYN_TERMS ? (long long)term_bytes : 0) - 1024;
+  return (int)std::min<long long>(std::max<long long>(room, 0) / 20 / 256 * 256, 8192);
+}
+template <int DIM, int ORD, int MAXU>
+int hcap_room_any(bool shaped, int device, size_t term_bytes) {
+  if (shaped) return hcap_room<DIM, ORD, MAXU, true>(device, term_bytes);
+  return hcap_room<DIM, ORD, MAXU, false>(device, term_bytes);
 }
 
 #define DISPATCH_U(D, O, nu, CALL) do { if ((nu) <= 32) { CALL(D, O, 1); } else { CALL(D, O, 4); } } while (0)
@@ -850,7 +864,7 @@ int batch_launch_tier(mplb_planner *p, BatchRun &R) {
   a.off_rows = L.off_rows; a.off_heap = L.off_heap; a.off_table = L.off_table; a.off_poplog = L.off_poplog;
   a.off_log = L.off_log; a.log_cap = L.log_cap;
   /* |U| > 32: when memory leaves at most one plan per SM anyway, that plan gets a much larger shared-memory heap top */
-  a.hcap = (c.nU > 32 && slots <= p->sm_count && p->hcap_big_cached > 0) ? p->hcap_big_cached : MPLB_HCAP_SMALL;
+  a.hcap = (c.nU > 32 && slots <= p->sm_count && p->hcap_big_cached > 0) ? p->hcap_big_cached : p->hcap_small_cached;
   a.want_poplog = R.retain ? 1 : 0; a.slot_of_plan = R.retain ? p->d_slot.p : nullptr;
   a.overflow_count = p->d_ctrl.p + 1; a.overflow_list = p->d_over.p;
 #ifdef MPLB_PHASE_TIMING
@@ -858,7 +872,7 @@ int batch_launch_tier(mplb_planner *p, BatchRun &R) {
   a.phase_cycles = p->d_phase.p;
 #endif
   const bool shaped = R.shaped;
-#define LAUNCH_CALL(D, O, M) rc = launch_any<D, O, M>(shaped, c, a, slots, s)
+#define LAUNCH_CALL(D, O, M) rc = launch_any<D, O, M>(shaped, c, a, p->term_bytes, slots, s)
   DISPATCH(c.dim, c.ord, c.nU, LAUNCH_CALL);
   if (rc != MPLB_OK) return rc;
   p->last_launches++; p->last_tiers++;
@@ -884,13 +898,23 @@ int run_batch_begin(mplb_planner *p, const mplb_waypoint *d_starts, const mplb_w
   if (retain) MPLB_CUDA_TRY(p->d_slot.reserve((size_t)n));
 
   /* resident CTAs of this kernel instantiation and the memory budget are looked up once per configuration: both
-   * calls cost on the order of a millisecond, comparable to a small batch */
+   * calls cost on the order of a millisecond, comparable to a small batch.  The term area of a |U| > 32 cost-shaping
+   * launch (dt, v_max, the map resolution and U decide it) takes shared memory from the heap top and from residency. */
   const bool shaped = c.pot != nullptr || c.region != nullptr || c.use_yaw != 0;
-  const int cfg_sig = (shaped ? 1000 : 0) + c.dim * 100 + c.ord * 10 + (c.nU <= 32 ? 1 : 4);
+  const long long cfg_sig = (long long)p->term_bytes * 10000 + (shaped ? 1000 : 0) + c.dim * 100 + c.ord * 10 + (c.nU <= 32 ? 1 : 4);
   if (p->resident_sig != cfg_sig) {
-    int r = 0;
-#define RES_CALL(D, O, M) do { r = resident_any<D, O, M>(shaped, p->device, MPLB_HCAP_SMALL); if (M > 1) p->hcap_big_cached = hcap_big<D, O, M>(p->device); } while (0)
+    int r = 0, room = 0;
+    /* heap top: MPLB_HCAP_SMALL entries when several plans share an SM, all the room there is with one plan per SM; the
+     * term area of a |U| > 32 cost-shaping launch can leave less than MPLB_HCAP_SMALL for either */
+#define RES_CALL(D, O, M)                                                                                             \
+  do {                                                                                                                \
+    if (M > 1) room = hcap_room_any<D, O, M>(shaped, p->device, p->term_bytes);                                        \
+    p->hcap_small_cached = (shaped && M > 1) ? std::min(MPLB_HCAP_SMALL, room) : MPLB_HCAP_SMALL;                      \
+    if (M > 1) p->hcap_big_cached = std::max(p->hcap_small_cached, room);                                              \
+    r = p->hcap_small_cached >= 256 ? resident_any<D, O, M>(shaped, p->device, p->hcap_small_cached, p->term_bytes) : 0; \
+  } while (0)
     DISPATCH(c.dim, c.ord, c.nU, RES_CALL);
+    if (p->hcap_small_cached < 256) return fail(MPLB_ERR_ARG, "the control set's sample terms leave no room for a shared-memory heap");
     p->resident_cached = r;
     p->resident_sig = cfg_sig;
   }
