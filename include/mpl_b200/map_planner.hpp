@@ -583,6 +583,40 @@ class MapPlanner {
     return mplb_lpa_sub_state_space_batch(h.data(), (int)n, ts.data(), sizes.data()) == MPLB_OK || batch_failed(planners);
   }
 
+  /* ---- the same fleet sharded over the ranks of `comm` (DESIGN.md section 6.1): `planners` are this rank's robots
+   * rank, rank + N, ... of n_total.  planLPAFleet is planLPABatch on them followed by mplb_fleet_plan's gather: on `root`,
+   * results / actions (may be NULL) receive every robot's record and first max_seg actions in robot order.  It is collective:
+   * every rank calls it with the same n_total, max_seg and root.  The cycle's map edit is mplb_fleet_map_edit on
+   * map_util_->handle() with the robots' device cell lists (INTEGRATION.md). */
+  static bool planLPAFleet(mplb_comm *comm, const std::vector<MapPlanner *> &planners, int n_total, const vec_E<Coord> &starts,
+                           const vec_E<Coord> &goals, std::vector<mplb_result> *results = nullptr,
+                           std::vector<int32_t> *actions = nullptr, int max_seg = 0, int root = 0) {
+    const size_t n = planners.size();
+    std::vector<mplb_planner *> h(n > 0 ? n : 1, nullptr);
+    std::vector<mplb_waypoint> s(n > 0 ? n : 1), g(n > 0 ? n : 1);
+    for (size_t i = 0; i < n; i++) {
+      MapPlanner *p = planners[i];
+      if (p->h_ && p->map_util_ && p->map_util_->handle() != p->bound_map_) p->setMapUtil(p->map_util_);
+      h[i] = p->h_; s[i] = to_c(starts[i]); g[i] = to_c(goals[i]);
+    }
+    const bool is_root = mplb_comm_rank(comm) == root;
+    const size_t n_res = is_root ? (size_t)n_total : n;
+    std::vector<mplb_result> res(n_res > 0 ? n_res : 1);
+    std::vector<int32_t> acts(is_root && max_seg > 0 ? (size_t)n_total * max_seg : 1, -1);
+    if (mplb_fleet_plan(comm, h.data(), (int)n, n_total, s.data(), g.data(), res.data(), acts.data(), max_seg, root) != MPLB_OK)
+      return batch_failed(planners);
+    const int N = mplb_comm_size(comm), r0 = mplb_comm_rank(comm);
+    for (size_t i = 0; i < n; i++) { /* the root's records are in robot order, the others' in local order */
+      MapPlanner *p = planners[i];
+      p->control_ = starts[i].control;
+      p->last_ = res[is_root ? (size_t)r0 + i * N : i];
+      p->planned();
+    }
+    if (is_root && results) results->assign(res.begin(), res.begin() + n_total);
+    if (is_root && actions && max_seg > 0) *actions = acts;
+    return true;
+  }
+
  private:
   /* plan()'s bookkeeping after the library planned into last_ */
   bool planned() {

@@ -478,6 +478,41 @@ int mplb_plan_batch_sharded_begin(mplb_planner *p, mplb_comm *c, const mplb_wayp
                                   int max_seg);
 int mplb_plan_batch_sharded_end(mplb_planner *p, mplb_comm *c, int n, mplb_result *results, int32_t *actions, int root);
 
+/* ---- a fleet of LPA* replanners over all ranks (DESIGN.md section 6.1): robot i of R lives on rank i mod N, as the queries of
+ * mplb_plan_batch_sharded, and every rank holds a replica of the shared map (mplb_comm_broadcast_map).  A cycle is the
+ * single-device fleet cycle of section 4.12.2 with two calls distributed: every rank calls both, with the same value / max_seg /
+ * root; getLinkedNodes, updateBlocked/ClearedNodes and getSubStateSpace stay rank-local (mplb_lpa_*_batch on the local robots).
+ *
+ * mplb_map_set_cells_device on every replica with the concatenation c_0 || c_1 || ... || c_{R-1} of all robots' edits.  This
+ * rank's n_local robots (its robots rank, rank + N, ... in order) own rows offsets_local[k] .. offsets_local[k+1]-1 of d_cells3
+ * (device rows of 3 ints, read once the work on `stream` (a cudaStream_t as void*, NULL = default) has completed; offsets_local
+ * is a host array of n_local + 1 entries).  One grouped ncclSend / ncclRecv exchange of a header and one of rows rebuild the
+ * concatenation in global robot order on every rank, independent of arrival order, in d_all_cells3 (device, `cap` rows of 3
+ * ints) with its R + 1 offsets in d_all_offsets (device int64), and every replica applies it.  Returns the concatenation's row
+ * count T.  Every rank passes the same cap: T <= cap means applied on every rank; T > cap means nothing was exchanged or
+ * applied anywhere (grow to T on every rank and call again).  With d_all_offsets = NULL on every rank the call is a size query:
+ * it returns T and applies nothing.  Every rank returns the same verdict: an argument error on any rank (null arguments, bad
+ * offsets, the map off the communicator's device), caps that differ, a size query on some ranks only, or robots per rank that do
+ * not follow the striping make every rank fail with MPLB_ERR_ARG.  Returns after the replica is written. */
+int64_t mplb_fleet_map_edit(mplb_comm *c, mplb_map *m, const void *d_cells3, const int64_t *offsets_local, int n_local, int value,
+                            void *d_all_cells3, void *d_all_offsets, int64_t cap, void *stream);
+/* mplb_lpa_plan_batch on this rank's n_local robots (grow-and-relaunch rounds included), then the gather of
+ * mplb_plan_batch_sharded: the root receives results[n_total] and, when max_seg > 0, actions[n_total * max_seg] (the first
+ * max_seg actions of each successful plan, -1 padded; -1 rows for the others) in robot order.  Every argument is checked before
+ * any planner changes, and their verdicts are exchanged first (one small grouped exchange) so that every rank fails alike: null
+ * arguments, a planner listed twice, a planner not on the communicator's device, n_local other than the number of robots the
+ * striping gives this rank, LPA* off, n_total or max_seg differing between ranks.  On the other ranks results may be NULL; when it is not, it
+ * receives their own n_local records in local order (actions is not written there). */
+/* The scan and merge of mplb_fleet_map_edit for a caller that moves the payloads with its own transport (MPI,
+ * torch.distributed): d_payloads holds the N ranks' payloads back to back (device int32 words; rank r's is payload_words[r]
+ * words: the per-robot row counts of its stripe_count robots of n_total, then their rows of 3 ints).  Writes the robot-ordered
+ * concatenation and its n_total + 1 offsets as mplb_fleet_map_edit does and returns its row count T (nothing written when
+ * T > cap); counts that do not add up to a payload's rows fail with MPLB_ERR_ARG.  Ordered on `stream`; returns when done. */
+int64_t mplb_fleet_merge_device(const void *d_payloads, const int64_t *payload_words, int nranks, int n_total, void *d_all_cells3,
+                                void *d_all_offsets, int64_t cap, void *stream);
+int mplb_fleet_plan(mplb_comm *c, mplb_planner **planners_local, int n_local, int n_total, const mplb_waypoint *starts_local,
+                    const mplb_waypoint *goals_local, mplb_result *results, int32_t *actions, int max_seg, int root);
+
 /* ---- VoxelGrid: the map builder of planning_ros_utils (include/planning_ros_utils/voxel_grid.h, src/mapping_utils/
  * voxel_grid.cpp, cited vg:<line>), the map store of mpl_test_node/src/cloud_to_map.cpp and map_replanner_node.cpp.  Both of
  * its int8 grids (map_ and inflated_map_) live on the device, x fastest, so a grid hands its map to an mplb_map without

@@ -135,6 +135,9 @@ SYMBOLS = {
     "mplb_lpa_update_nodes_batch": (_I, [_VP, _I, _I, _VP, _VP, _VP]),
     "mplb_lpa_update_nodes_batch_device": (_I, [_VP, _I, _I, _VP, _VP, _VP]),
     "mplb_lpa_sub_state_space_batch": (_I, [_VP, _I, _VP, _VP]),
+    "mplb_fleet_map_edit": (C.c_int64, [_VP, _VP, _VP, _VP, _I, _I, _VP, _VP, C.c_int64, _VP]),
+    "mplb_fleet_merge_device": (C.c_int64, [_VP, _VP, _I, _I, _VP, _VP, C.c_int64, _VP]),
+    "mplb_fleet_plan": (_I, [_VP, _VP, _I, _I, _VP, _VP, _VP, _VP, _I, _I]),
 }
 TRACE_ALL, TRACE_FREE, TRACE_OCCUPIED = 0, 1, 2  # mplb_map_trace_cells selections
 

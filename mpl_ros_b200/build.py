@@ -15,6 +15,7 @@ UNITS = {
     "mplb_trajsolve.cu": [os.path.join(CSRC, "mplb_ref.h")] + _COMMON,
     "mplb_lpa.cu": [os.path.join(CSRC, h) for h in ("mplb_lpa_core.h", "mplb_ref.h")] + _COMMON,
     "mplb_voxel.cu": [os.path.join(CSRC, "mplb_ref.h")] + _COMMON,
+    "mplb_fleet.cu": _COMMON,
 }
 DEPS = [SRC] + UNITS["mplb.cu"]
 OUT = os.path.join(HERE, "libmplb.so")

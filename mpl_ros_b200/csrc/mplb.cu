@@ -1918,6 +1918,7 @@ struct mplb_comm {
   int rank = 0, nranks = 1, device = 0;
   cudaStream_t stream = nullptr;
   DevBuf<unsigned char> gres, gact, hdr; /* gather buffers on the root, header scratch */
+  DevBuf<unsigned char> fleet[MPLB_COMM_FLEET_SLOTS]; /* grow-only scratch of the fleet calls (mplb_fleet.cu) */
 };
 
 int mplb_comm_unique_id(uint8_t *id128) {
@@ -1995,9 +1996,41 @@ int mplb_comm_broadcast_map(mplb_comm *c, int root, int dim, const int32_t *ndim
   return MPLB_OK;
 }
 
+void mplb_internal_comm_view(mplb_comm *c, MplbCommView *out) {
+  out->rank = c->rank; out->nranks = c->nranks; out->device = c->device; out->stream = c->stream;
+}
+
+void *mplb_internal_comm_scratch(mplb_comm *c, int slot, size_t bytes) {
+  DevBuf<unsigned char> &b = c->fleet[slot];
+  if (b.n < bytes && b.reserve(std::max<size_t>(bytes, 2 * b.n)) != cudaSuccess) {
+    mplb_internal_fail(MPLB_ERR_CUDA, "fleet scratch allocation failed");
+    return nullptr;
+  }
+  return b.p;
+}
+
+int mplb_internal_comm_allgather(mplb_comm *c, const void *send, const size_t *bytes, void *recv, void *stream) {
+  NcclApi &N = nccl_api();
+  cudaStream_t s = (cudaStream_t)stream;
+  std::vector<size_t> off(c->nranks + 1, 0);
+  for (int r = 0; r < c->nranks; r++) off[r + 1] = off[r] + bytes[r];
+  unsigned char *out = (unsigned char *)recv;
+  if (bytes[c->rank]) MPLB_CUDA_TRY(cudaMemcpyAsync(out + off[c->rank], send, bytes[c->rank], cudaMemcpyDeviceToDevice, s));
+  if (c->nranks == 1) return MPLB_OK;
+  NCCL_TRY(N.GroupStart());
+  for (int r = 0; r < c->nranks; r++) { /* every rank knows every size: a zero-byte leg is skipped on both of its ends */
+    if (r == c->rank) continue;
+    if (bytes[c->rank]) NCCL_TRY(N.Send(send, bytes[c->rank], ncclUint8, r, c->comm, s));
+    if (bytes[r]) NCCL_TRY(N.Recv(out + off[r], bytes[r], ncclUint8, r, c->comm, s));
+  }
+  NCCL_TRY(N.GroupEnd());
+  return MPLB_OK;
+}
+
 /* gather of this rank's `per` result records and action rows (device buffers) into the root's gather buffers:
  * one ncclGroup of sends/receives */
-static int comm_gather(mplb_comm *c, const void *d_res, const void *d_act, int per, int max_seg, int root, cudaStream_t s) {
+int mplb_internal_comm_gather(mplb_comm *c, const void *d_res, const void *d_act, int per, int max_seg, int root, void *stream) {
+  const cudaStream_t s = (cudaStream_t)stream;
   NcclApi &N = nccl_api();
   const size_t rb = (size_t)per * sizeof(mplb_result), ab = (size_t)per * max_seg * sizeof(int);
   if (c->rank == root) {
@@ -2034,7 +2067,7 @@ int mplb_plan_stripe_gather_device(mplb_planner *p, mplb_comm *c, const void *d_
   int rc = MPLB_OK;
   if (n_local > 0) rc = mplb_plan_batch_device(p, d_starts, d_goals, n_local, d_results, d_actions, nullptr, max_seg, stream);
   if (rc != MPLB_OK) return rc;
-  rc = comm_gather(c, d_results, max_seg > 0 ? d_actions : nullptr, per, max_seg > 0 ? max_seg : 0, root, (cudaStream_t)stream);
+  rc = mplb_internal_comm_gather(c, d_results, max_seg > 0 ? d_actions : nullptr, per, max_seg > 0 ? max_seg : 0, root, stream);
   if (rc != MPLB_OK) return rc;
   MPLB_CUDA_TRY(cudaStreamSynchronize((cudaStream_t)stream));
   return MPLB_OK;
@@ -2066,7 +2099,7 @@ int mplb_plan_stripe_end(mplb_planner *p, mplb_comm *c, int per, int root) {
   if (rc != MPLB_OK) return rc;
   /* every gather of a communicator runs on the communicator's stream, in call order (the search is complete: run_batch_end
    * synchronised the planner's stream) */
-  rc = comm_gather(c, p->run->d_results, p->run->max_seg > 0 ? p->run->d_actions : nullptr, per, p->run->max_seg > 0 ? p->run->max_seg : 0, root,
+  rc = mplb_internal_comm_gather(c, p->run->d_results, p->run->max_seg > 0 ? p->run->d_actions : nullptr, per, p->run->max_seg > 0 ? p->run->max_seg : 0, root,
                    c->stream);
   if (rc != MPLB_OK) return rc;
   MPLB_CUDA_TRY(cudaStreamSynchronize(c->stream));
@@ -2106,7 +2139,7 @@ int mplb_plan_batch_sharded_end(mplb_planner *p, mplb_comm *c, int n, mplb_resul
   if (p->async_n > 0) rc = run_batch_end(p);
   if (rc != MPLB_OK) return rc;
   const int ms = p->async_ms;
-  rc = comm_gather(c, p->d_results.p, ms > 0 ? p->d_actions.p : nullptr, p->async_per, ms > 0 ? ms : 0, root, c->stream);
+  rc = mplb_internal_comm_gather(c, p->d_results.p, ms > 0 ? p->d_actions.p : nullptr, p->async_per, ms > 0 ? ms : 0, root, c->stream);
   if (rc != MPLB_OK) return rc;
   MPLB_CUDA_TRY(cudaStreamSynchronize(c->stream));
   if (c->rank == root) return mplb_comm_unstripe(c, n, p->async_per, actions ? ms : 0, results, actions);

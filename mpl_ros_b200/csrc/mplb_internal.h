@@ -113,4 +113,24 @@ struct MplbMapView {
 MPLB_HIDDEN void mplb_internal_map_view(mplb_map *m, MplbMapView *out);
 /* after d_grid was rewritten on `stream` (a cudaStream_t): rebuild the occupancy bit-bricks, as mplb_map_set_data does */
 MPLB_HIDDEN int mplb_internal_map_cells_changed(mplb_map *m, void *stream);
+
+/* ---- what the fleet unit (mplb_fleet.cu) needs from the communicator of mplb.cu (defined in its extern "C" block) */
+struct MplbCommView {
+  int rank, nranks, device;
+  void *stream; /* the communicator's cudaStream_t: every collective of a communicator runs on it, in call order */
+};
+extern "C" {
+MPLB_HIDDEN void mplb_internal_comm_view(mplb_comm *c, MplbCommView *out);
+/* at least `bytes` bytes of the communicator's grow-only scratch slot `slot` (< MPLB_COMM_FLEET_SLOTS) on its device, kept until
+ * the communicator is destroyed; contents are not kept when it grows.  NULL (mplb_last_error set) when it cannot be allocated. */
+#define MPLB_COMM_FLEET_SLOTS 8
+MPLB_HIDDEN void *mplb_internal_comm_scratch(mplb_comm *c, int slot, size_t bytes);
+/* rank r's bytes[r] bytes (device memory; `send` is this rank's) land at recv + bytes[0] + ... + bytes[r - 1] on every
+ * rank: one group of ncclSend / ncclRecv on `stream`, enqueued only.  Every rank passes the same sizes. */
+MPLB_HIDDEN int mplb_internal_comm_allgather(mplb_comm *c, const void *send, const size_t *bytes, void *recv, void *stream);
+/* this rank's `per` result records and action rows (device buffers) into the root's gather buffers, which
+ * mplb_comm_unstripe reads: one group of ncclSend / ncclRecv on `stream`, enqueued only */
+MPLB_HIDDEN int mplb_internal_comm_gather(mplb_comm *c, const void *d_res, const void *d_act, int per, int max_seg, int root,
+                                          void *stream);
+}
 #endif

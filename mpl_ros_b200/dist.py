@@ -302,3 +302,183 @@ class ShardedBatchPlanner:
         res, acts, _ = self.planner.plan_batch(np.ascontiguousarray(starts[idx]), np.ascontiguousarray(goals[idx]),
                                                max_seg=max_seg)
         return gather_results(res, acts, len(starts), max_seg, self.device, dst)
+
+
+# ---- a fleet of LPA* replanners sharded over ranks (mplb_fleet_map_edit / mplb_fleet_plan, DESIGN.md section 6.1): robot i lives
+# on rank i mod N; every rank holds a replica of the shared map.  A replan cycle is the single-device fleet cycle with the map
+# edit and the plan distributed: every replica applies the concatenation of all robots' edits in robot order, and the plans
+# come back to one root in robot order.
+
+def _rows3(cells):
+    """rows of 2 or 3 ints -> rows of 3 int32 (the third 0 in 2D)"""
+    c = np.asarray(cells, dtype=np.int32).reshape(len(cells), -1) if len(cells) else np.zeros((0, 3), dtype=np.int32)
+    out = np.zeros((len(c), 3), dtype=np.int32)
+    out[:, :c.shape[1]] = c
+    return out
+
+
+def pack_edits(cells_local):
+    """This rank's robots' edit lists -> (per-robot row counts int64, rows int32 [k, 3]): the send payload of the exchange."""
+    c3 = [np.asarray(c, dtype=np.int32).reshape(-1, 3) for c in cells_local]
+    counts = np.array([len(c) for c in c3], dtype=np.int64)
+    rows = np.concatenate(c3) if c3 else np.zeros((0, 3), dtype=np.int32)
+    return counts, np.ascontiguousarray(rows, dtype=np.int32)
+
+
+def merge_edits(parts, n_total):
+    """The received payloads (counts, rows) of ranks 0 .. N-1 -> the concatenation c_0 || ... || c_{R-1} in robot order (robot i
+    = the (i / N)-th robot of rank i mod N) and its R + 1 offsets.  Independent of the order the payloads arrived in."""
+    world = len(parts)
+    starts = [np.concatenate([[0], np.cumsum(c)]).astype(np.int64) for c, _ in parts]
+    lists, offs = [], np.zeros(n_total + 1, dtype=np.int64)
+    for i in range(n_total):
+        r, k = i % world, i // world
+        lists.append(parts[r][1][starts[r][k]:starts[r][k + 1]])
+        offs[i + 1] = offs[i] + len(lists[-1])
+    cells = np.concatenate(lists) if lists else np.zeros((0, 3), dtype=np.int32)
+    return np.ascontiguousarray(cells, dtype=np.int32).reshape(-1, 3), offs
+
+
+def exchange_edits(cells_local, n_total, device):
+    """torch.distributed stand-in of mplb_fleet_map_edit's exchange (gloo on a CPU box): one all-gather of the payload sizes,
+    one of the payloads (padded to the largest), then merge_edits.  Returns (cells [T, 3] int32, offsets [R + 1]) on every rank."""
+    rank, world = _rank_world()
+    counts, rows = pack_edits(cells_local)
+    if world == 1:
+        return merge_edits([(counts, rows)], n_total)
+    words = np.concatenate([counts.astype(np.int32), rows.reshape(-1)]).astype(np.int32)
+    size = torch.tensor([len(counts), len(rows)], dtype=torch.int64, device=device)
+    sizes = [torch.empty_like(size) for _ in range(world)]
+    dist.all_gather(sizes, size)
+    sizes = [tuple(int(v) for v in s.cpu().numpy()) for s in sizes]
+    width = max(max(n + 3 * k for n, k in sizes), 1)
+    buf = torch.zeros(width, dtype=torch.int32, device=device)
+    buf[:len(words)] = torch.as_tensor(words)
+    bufs = [torch.empty_like(buf) for _ in range(world)]
+    dist.all_gather(bufs, buf)
+    parts = []
+    for (n, k), b in zip(sizes, bufs):
+        w = b.cpu().numpy()
+        parts.append((w[:n].astype(np.int64), w[n:n + 3 * k].reshape(k, 3)))
+    return merge_edits(parts, n_total)
+
+
+class ShardedFleet:
+    """This rank's robots of a fleet of R LPA* replanners (robot i on rank i mod N) and one replan cycle over all ranks.
+
+    planners: this rank's MapPlanner objects (LPA* on), robots rank, rank + N, ... in that order.  map_util: this rank's replica
+    of the shared map (None for a fleet whose robots each own a map: then only the plan is collective).  With `comm` (a dist.Comm)
+    the edit and the gather run inside libmplb on the device; without it the default torch.distributed group carries them
+    (gloo works), and `_set_cells` / `_plan_local` do the rank-local work, which a CPU test may replace with stand-ins."""
+
+    def __init__(self, planners, n_total, map_util=None, comm=None, device=None):
+        self.planners, self.n_total, self.map_util, self.comm, self.device = list(planners), int(n_total), map_util, comm, device
+        self.rank, self.world = (comm.rank, comm.size) if comm is not None else _rank_world()
+        self.local = shard_indices(self.n_total, self.rank, self.world)
+        if len(self.local) != len(self.planners):
+            raise ValueError("rank %d of %d holds robots %s of %d, not %d planners" % (self.rank, self.world, list(self.local),
+                                                                                      self.n_total, len(self.planners)))
+        self.cells, self.offsets = np.zeros((0, 3), dtype=np.int32), np.zeros(self.n_total + 1, dtype=np.int64)
+        self._d_all = self._d_off = None
+        self._T = 0
+
+    # ---- step 1 and 2: every robot's edit reaches every replica, in robot order
+    def map_edit(self, cells_local, value):
+        """cells_local[k]: the edit of this rank's k-th robot (rows of 2 or 3 ints).  Every replica receives
+        mplb_map_set_cells(c_0 || ... || c_{R-1}, value).  Returns the row count T of that concatenation, which stays on the
+        device for update(); edit_cells() / edit_offsets() copy it and its R + 1 offsets to the host."""
+        c3 = [_rows3(c) for c in cells_local]
+        if self.comm is None:
+            self.cells, self.offsets = exchange_edits(c3, self.n_total, self.device)
+            self._T = len(self.cells)
+            if self._T:
+                self._set_cells(self.cells, value)
+            return self._T
+        import ctypes as C
+        counts, rows = pack_edits(c3)
+        offs = np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)
+        d_rows = torch.as_tensor(rows).to(self.device) if len(rows) else None
+        vp = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None  # noqa: E731
+        if self._d_off is None:
+            self._d_off = torch.zeros(self.n_total + 1, dtype=torch.int64, device=self.device)
+            self._d_all = torch.zeros((1024, 3), dtype=torch.int32, device=self.device)
+        stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)  # the stream d_rows was written on
+        for _ in range(2):  # every rank holds the same cap, so T > cap on one rank is T > cap on all: all grow and call again
+            total = _lib.check(_lib.lib().mplb_fleet_map_edit(self.comm._h, self.map_util._h, vp(d_rows), _lib.ptr(offs), len(c3),
+                                                             int(value), vp(self._d_all), vp(self._d_off), self._d_all.shape[0], stream))
+            if total <= self._d_all.shape[0]:
+                break
+            self._d_all = torch.zeros((total, 3), dtype=torch.int32, device=self.device)
+        self._T = total
+        return total
+
+    def edit_cells(self):
+        """the last map_edit's concatenation c_0 || ... || c_{R-1}, rows of 3 int32 on the host"""
+        return self.cells if self.comm is None else self._d_all[:self._T].cpu().numpy()
+
+    def edit_offsets(self):
+        """its R + 1 offsets on the host: robot i's rows are edit_cells()[offsets[i]:offsets[i + 1]]"""
+        return self.offsets if self.comm is None else self._d_off.cpu().numpy()
+
+    def _set_cells(self, cells, value):
+        self.map_util.setCells(cells, value)
+
+    # ---- steps 3 to 6: rank-local, except the gather of the plans
+    def links(self):
+        from .planner import MapPlanner
+        return MapPlanner.getLinkedNodesBatch(self.planners)
+
+    def update(self, blocked, selection=None):
+        """updateBlockedNodes (blocked) / updateClearedNodes of this rank's robots: by default every robot receives the whole
+        concatenation of the last map_edit; selection[k] (rows of ints) replaces it for this rank's k-th robot."""
+        from .planner import MapPlanner
+        if selection is not None:
+            return MapPlanner._update_batch(self.planners, selection, blocked)
+        n, T = len(self.planners), self._T
+        if self.comm is None or n == 0:
+            return MapPlanner._update_batch(self.planners, [self.cells] * n, blocked)
+        import ctypes as C
+        # The batched update gives entry k the rows offsets[k] .. offsets[k+1]-1, so one list cannot be shared by several
+        # entries: the device concatenation is repeated once per local robot (n T rows of 12 B), and entry k reads copy k.
+        rep = self._d_all[:T].repeat(n, 1) if T else None
+        offs = (np.arange(n + 1, dtype=np.int64) * T)
+        torch.cuda.current_stream(self.device).synchronize()  # the update reads `rep` on the default stream
+        visited = np.zeros(n, dtype=np.int32)
+        _lib.check(_lib.lib().mplb_lpa_update_nodes_batch_device(MapPlanner._handles(self.planners), n, int(blocked),
+                                                                 C.c_void_p(rep.data_ptr()) if rep is not None else None,
+                                                                 _lib.ptr(offs), _lib.ptr(visited)))
+        return [int(v) for v in visited]
+
+    def plan(self, starts_local, goals_local, max_seg=64, root=0):
+        """planLPABatch of this rank's robots, gathered: (results[R], actions[R, max_seg]) in robot order on `root`, (None, None)
+        elsewhere.  Every local planner keeps result(), traj_ and traj_cost_ as plan() does."""
+        if self.comm is not None:
+            from .planner import MapPlanner
+            return MapPlanner.planLPAFleet(self.comm, self.planners, self.n_total, starts_local, goals_local, max_seg, root)
+        res, acts = self._plan_local(starts_local, goals_local, max_seg)
+        return gather_results(res, acts, self.n_total, max_seg, self.device, root)
+
+    def _plan_local(self, starts, goals, max_seg):
+        from .planner import MapPlanner
+        n = len(self.planners)
+        MapPlanner.planLPABatch(self.planners, starts, goals)
+        res = np.zeros(n, dtype=_lib.RESULT_DTYPE)
+        acts = np.full((n, max_seg), -1, dtype=np.int32)
+        for k, pl in enumerate(self.planners):
+            res[k] = pl.result()
+            if int(res[k]["status"]) == 0 and max_seg:
+                a = pl.getActions()[:max_seg]
+                acts[k, :len(a)] = a
+        return res, acts
+
+    def sub_state_space(self, time_steps_local):
+        from .planner import MapPlanner
+        return MapPlanner.getSubStateSpaceBatch(self.planners, time_steps_local)
+
+    def cycle(self, cells_local, value, starts_local, goals_local, time_steps_local, selection=None, max_seg=64, root=0):
+        """One replan cycle: edit, getLinkedNodes, update, plan, getSubStateSpace.  Returns the gathered plan (root) and sizes."""
+        self.map_edit(cells_local, value)
+        self.links()
+        self.update(value == 100, selection)
+        out = self.plan(starts_local, goals_local, max_seg, root)
+        return out, self.sub_state_space(time_steps_local)

@@ -528,6 +528,29 @@ class MapPlanner:
         return [pl._planned(res[i], int(s["control"][i])) for i, pl in enumerate(planners)]
 
     @staticmethod
+    def planLPAFleet(comm, planners, n_total, starts, goals, max_seg=64, root=0):
+        """mplb_fleet_plan: planLPABatch of this rank's robots (planners: robots rank, rank + N, ... of n_total, on comm's
+        device), gathered through comm (a dist.Comm).  Returns (results[n_total], actions[n_total, max_seg]) in robot order on
+        `root`, (None, None) elsewhere; every local planner keeps result(), traj_ and traj_cost_ as plan() does."""
+        n = len(planners)
+        s, g = waypoints_array(n), waypoints_array(n)
+        for i in range(n):
+            for src, dst in ((starts[i], s), (goals[i], g)):
+                if isinstance(src, Waypoint):
+                    src.to_record(dst[i])
+                else:
+                    dst[i] = np.asarray(src).reshape(-1)[0] if np.ndim(src) else src
+        is_root = comm.rank == root
+        res = np.zeros(max(n_total if is_root else n, 1), dtype=_lib.RESULT_DTYPE)
+        acts = np.full((max(n_total, 1), max(max_seg, 1)), -1, dtype=np.int32) if is_root else None
+        check(lib().mplb_fleet_plan(comm._h, MapPlanner._handles(planners), n, int(n_total), ptr(s), ptr(g), ptr(res), ptr(acts),
+                                    int(max_seg), int(root)))
+        own = np.arange(comm.rank, n_total, comm.size) if is_root else np.arange(n)  # the root's records are in robot order
+        for k, pl in enumerate(planners):
+            pl._planned(res[own[k]], int(s["control"][k]))
+        return (res[:n_total], acts[:n_total, :max_seg]) if is_root else (None, None)
+
+    @staticmethod
     def getLinkedNodesBatch(planners):
         """getLinkedNodes of every planner (mplb_lpa_get_linked_nodes_batch): a list of (k_i, Dim) point arrays"""
         n = len(planners)
