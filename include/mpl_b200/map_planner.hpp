@@ -583,6 +583,46 @@ class MapPlanner {
     return mplb_lpa_sub_state_space_batch(h.data(), (int)n, ts.data(), sizes.data()) == MPLB_OK || batch_failed(planners);
   }
 
+  /* ---- the cycle's output on the device (mplb.h: mplb_lpa_plan_batch_device and the calls after it).  Buffers are device
+   * pointers on the planners' device, `stream` a cudaStream_t (NULL = default); each call returns after its work completed.
+   * planLPABatchDevice leaves the library's retained trajectory as plan() does (getActions / getSegStates), but not this
+   * object's last_ / traj_ / traj_cost_: nothing is read back. */
+  static bool planLPABatchDevice(const std::vector<MapPlanner *> &planners, const void *d_starts, const void *d_goals, void *d_results,
+                                 void *d_actions, void *d_seg_states, int max_seg, void *stream = nullptr) {
+    std::vector<mplb_planner *> h = bound_handles(planners);
+    return mplb_lpa_plan_batch_device(h.data(), (int)planners.size(), d_starts, d_goals, d_results, d_actions, d_seg_states, max_seg,
+                                      stream) == MPLB_OK || batch_failed(planners);
+  }
+  /* getTraj().getWaypoints()[d_index[i]] of plan i (the replanner node's next start), d_ok[i] = 0 where there is none */
+  static bool trajectoryWaypointsBatch(const std::vector<MapPlanner *> &planners, const void *d_results, const void *d_actions,
+                                       const void *d_seg_states, int max_seg, const void *d_index, void *d_waypoints, void *d_ok,
+                                       void *stream = nullptr) {
+    std::vector<mplb_planner *> h = handles(planners);
+    return mplb_lpa_trajectory_waypoints_device(h.data(), (int)planners.size(), d_results, d_actions, d_seg_states, max_seg, d_index,
+                                                d_waypoints, d_ok, stream) == MPLB_OK || batch_failed(planners);
+  }
+  /* toTrajectoryROSMsg + the wire bytes of every plan, plan i with planner i's own controls and dt */
+  static bool serializeLPABatch(const std::vector<MapPlanner *> &planners, const void *d_results, const void *d_actions,
+                                const void *d_seg_states, int max_seg, void *d_out, size_t stride, void *d_len, double z = 0.0,
+                                const char *frame_id = "map", uint32_t seq = 0, uint32_t stamp_sec = 0, uint32_t stamp_nsec = 0,
+                                void *stream = nullptr) {
+    std::vector<mplb_planner *> h = handles(planners);
+    return mplb_lpa_serialize_trajectories_device(h.data(), (int)planners.size(), d_results, d_actions, d_seg_states, max_seg, z, seq,
+                                                  stamp_sec, stamp_nsec, frame_id, d_out, stride, d_len, stream) == MPLB_OK ||
+           batch_failed(planners);
+  }
+  /* map_planner_node.cpp:216-227 for every plan (coefficient rows [n][max_seg][Dim + 1][6]); n_segs may be NULL */
+  static bool refineLPABatch(const std::vector<MapPlanner *> &planners, const void *d_results, const void *d_actions,
+                             const void *d_seg_states, int max_seg, void *d_coefs, std::vector<int32_t> *n_segs = nullptr,
+                             int control = MPLB_CONTROL_JRK, int yaw_control = MPLB_CONTROL_VEL, void *stream = nullptr) {
+    std::vector<mplb_planner *> h = handles(planners);
+    std::vector<int32_t> ns(planners.size() > 0 ? planners.size() : 1, 0);
+    const bool ok = mplb_lpa_refine_trajectories_device(h.data(), (int)planners.size(), d_results, d_actions, d_seg_states, max_seg,
+                                                        control, yaw_control, d_coefs, ns.data(), stream) == MPLB_OK;
+    if (ok && n_segs) n_segs->assign(ns.begin(), ns.begin() + planners.size());
+    return ok || batch_failed(planners);
+  }
+
   /* ---- the same fleet sharded over the ranks of `comm` (DESIGN.md section 6.1): `planners` are this rank's robots
    * rank, rank + N, ... of n_total.  planLPAFleet is planLPABatch on them followed by mplb_fleet_plan's gather: on `root`,
    * results / actions (may be NULL) receive every robot's record and first max_seg actions in robot order.  It is collective:
@@ -642,6 +682,11 @@ class MapPlanner {
     std::vector<mplb_planner *> h(planners.size() > 0 ? planners.size() : 1, nullptr);
     for (size_t i = 0; i < planners.size(); i++) h[i] = planners[i]->h_;
     return h;
+  }
+  static std::vector<mplb_planner *> bound_handles(const std::vector<MapPlanner *> &planners) { /* as planLPABatch binds the map */
+    for (MapPlanner *p : planners)
+      if (p->h_ && p->map_util_ && p->map_util_->handle() != p->bound_map_) p->setMapUtil(p->map_util_);
+    return handles(planners);
   }
   static bool batch_failed(const std::vector<MapPlanner *> &planners) {
     if (!planners.empty()) planners[0]->report();

@@ -341,6 +341,44 @@ int mplb_update_cleared_nodes(mplb_planner *p, const int32_t *cells3, int n);
  * trajectory of any length for mplb_get_actions / mplb_get_seg_states.  A session that has to grow stops before the pop that
  * could overflow; the host doubles its arrays and relaunches the batch, in which finished sessions return at once. */
 int mplb_lpa_plan_batch(mplb_planner **planners, int n, const mplb_waypoint *starts, const mplb_waypoint *goals, mplb_result *results);
+/* ---- a fleet cycle's output on the device (DESIGN.md section 4.12.3, "The cycle's output on the device").
+ * mplb_lpa_plan_batch_device: mplb_lpa_plan_batch with DEVICE starts / goals [n] and results [n] on the planners' device, ordered on
+ * `stream` (cudaStream_t as void*, NULL = default); returns after the batch has completed.  Entry i behaves exactly like
+ * mplb_lpa_plan_batch for planner i (record, state space, growth and resume, the retained trajectory of mplb_get_actions /
+ * mplb_get_seg_states, which a failed plan leaves as it was).  Nothing is read back for the caller: bindings that keep a host-side
+ * record of the last plan (the Python and C++ result() / getTraj() / getTrajCost()) still show the last plan made through the host
+ * calls, while mplb_get_actions / mplb_get_seg_states and the mplb_lpa_get_* dumps show this one.  Plan i's trajectory goes to d_actions[i*max_seg ..] and
+ * d_seg_states[(i*max_seg ..)*13], the layout of mplb_plan_batch_device: the true n_seg is reported, only the first max_seg rows are
+ * written, action rows past the trajectory (all of them for a failed plan) are -1 and seg-state rows past it are not written.
+ * d_actions / d_seg_states may be NULL.  Fails with no planner touched on a null argument, a planner listed twice, LPA* off, planners
+ * on different devices or max_seg < 0.  The host work of a call does not grow with n. */
+int mplb_lpa_plan_batch_device(mplb_planner **planners, int n, const void *d_starts, const void *d_goals, void *d_results,
+                               void *d_actions, void *d_seg_states, int max_seg, void *stream);
+/* The next starts of map_replanner_node.cpp:243-253 (start = traj.getWaypoints()[1] after getSubStateSpace): for the plan-batch
+ * layout above (same planners, same order, max_seg >= 1), d_waypoints[i] = Trajectory::getWaypoints()[d_index[i]]
+ * (trajectory.h:277-289) of plan i as an mplb_waypoint: waypoint j < n_seg is segment j's stored parent coord, waypoint n_seg the
+ * last primitive evaluated at dt in the reference's term order; t is the running sum 0 + dt + ... + dt of getWaypoints, control
+ * the plan's control flags.  d_index: int32 [n] (device); d_ok: int32 [n] (device), 1 where a waypoint was written, 0 (and
+ * d_waypoints[i] untouched) where the plan failed, n_seg > max_seg or d_index[i] is outside [0, n_seg].  The output can be passed
+ * to mplb_lpa_plan_batch_device as the next cycle's starts.  Returns after the kernel has completed. */
+int mplb_lpa_trajectory_waypoints_device(mplb_planner **planners, int n, const void *d_results, const void *d_actions,
+                                         const void *d_seg_states, int max_seg, const void *d_index, void *d_waypoints, void *d_ok,
+                                         void *stream);
+/* mplb_serialize_trajectories_device (toTrajectoryROSMsg, map_planner_node / map_replanner_node.cpp:124-130,158-164) and
+ * mplb_refine_trajectories_device for the plan-batch layout above: entry i is read with planner i's own dim, control order, yaw
+ * flag, controls and dt of its last LPA* plan, so one call serves a fleet of differently configured robots and no A* batch is
+ * needed.  Bytes, lengths, coefficient rows and n_segs are those the A* forms give for the same rows and configuration (frame,
+ * header, z, stride, truncation and len = 0 rules unchanged; refine: plan_control is each plan's own, every planner of one call
+ * must plan in the same dim, and control / yaw_control are the solver orders of the whole call).  Both fail before writing
+ * anything on a null argument, a planner listed twice, a planner without LPA* or without a plan, or planners on different
+ * devices, and return after their work has completed. */
+int mplb_lpa_serialize_trajectories_device(mplb_planner **planners, int n, const void *d_results, const void *d_actions,
+                                           const void *d_seg_states, int max_seg, double z, uint32_t seq, uint32_t stamp_sec,
+                                           uint32_t stamp_nsec, const char *frame_id, void *d_out, size_t stride, void *d_len,
+                                           void *stream);
+int mplb_lpa_refine_trajectories_device(mplb_planner **planners, int n, const void *d_results, const void *d_actions,
+                                        const void *d_seg_states, int max_seg, int control, int yaw_control, void *d_coefs,
+                                        int32_t *n_segs, void *stream);
 /* The rest of a replan cycle for many replanners per call.  Entry i leaves planners[i] exactly as the single call of the same
  * member would, and reports what that call returns.  Every call checks all of its arguments first and fails with no planner
  * touched when one is null, a planner appears twice, a planner has LPA* off or has not planned, the planners live on

@@ -138,6 +138,11 @@ SYMBOLS = {
     "mplb_fleet_map_edit": (C.c_int64, [_VP, _VP, _VP, _VP, _I, _I, _VP, _VP, C.c_int64, _VP]),
     "mplb_fleet_merge_device": (C.c_int64, [_VP, _VP, _I, _I, _VP, _VP, C.c_int64, _VP]),
     "mplb_fleet_plan": (_I, [_VP, _VP, _I, _I, _VP, _VP, _VP, _VP, _I, _I]),
+    "mplb_lpa_plan_batch_device": (_I, [_VP, _I, _VP, _VP, _VP, _VP, _VP, _I, _VP]),
+    "mplb_lpa_trajectory_waypoints_device": (_I, [_VP, _I, _VP, _VP, _VP, _I, _VP, _VP, _VP, _VP]),
+    "mplb_lpa_serialize_trajectories_device": (_I, [_VP, _I, _VP, _VP, _VP, _I, _D, C.c_uint32, C.c_uint32, C.c_uint32, C.c_char_p,
+                                                    _VP, C.c_size_t, _VP, _VP]),
+    "mplb_lpa_refine_trajectories_device": (_I, [_VP, _I, _VP, _VP, _VP, _I, _I, _I, _VP, _VP, _VP]),
 }
 TRACE_ALL, TRACE_FREE, TRACE_OCCUPIED = 0, 1, 2  # mplb_map_trace_cells selections
 

@@ -198,9 +198,10 @@ struct MsgArgs {
   const mplb_result *results;
   const int *actions;
   const double *segs;
-  int n, max_seg, dim, ord, use_yaw;
-  const double *U, *Uyaw;
-  double dt, z;
+  int n, max_seg;
+  const MplbTrajCfg *cfgs; /* plan i's dim, order, yaw flag, controls and dt: cfgs[cfg_id ? cfg_id[i] : 0] */
+  const int *cfg_id;
+  double z;
   unsigned seq, sec, nsec, frame_len;
   unsigned char frame[64];
   unsigned char *out;
@@ -216,6 +217,7 @@ __global__ void k_serialize_traj(const __grid_constant__ MsgArgs a) {
   for (long long w = (long long)blockIdx.x * wpb + (threadIdx.x >> 5); w < total; w += (long long)gridDim.x * wpb) {
     const int plan = (int)(w / (a.max_seg + 1)), k = (int)(w % (a.max_seg + 1)) - 1;
     const mplb_result r = a.results[plan];
+    const MplbTrajCfg c = a.cfgs[a.cfg_id ? a.cfg_id[plan] : 0];
     const int n_seg = (r.status == MPLB_PLAN_OK) ? r.n_seg : 0;
     const size_t head = 16 + (size_t)a.frame_len + 4; /* seq, stamp.sec, stamp.nsec, frame_id length + bytes, primitive count */
     const size_t need = head + (size_t)n_seg * 216 + 4;
@@ -243,20 +245,20 @@ __global__ void k_serialize_traj(const __grid_constant__ MsgArgs a) {
     unsigned char *po = o + head + (size_t)k * 216;
     for (int b = lane; b < 216; b += 32) {
       unsigned char v;
-      if (b >= 208) v = byte_of(a.dt, b - 208);
+      if (b >= 208) v = byte_of(c.dt, b - 208);
       else {
         const int arr = b / 52, off = b % 52; /* arr: 0 cx, 1 cy, 2 cz, 3 cyaw */
         if (off < 4) v = byte_of(6u, off);
         else {
           const int ci = (off - 4) >> 3, bb = (off - 4) & 7; /* coefficient index 0..5, highest order first (pr:35-52) */
-          double c = 0.0;
-          if (arr < a.dim) {
+          double x = 0.0;
+          if (arr < c.dim) {
             const int d = 5 - ci; /* derivative held by this coefficient */
-            if (d < a.ord) c = row[d * 3 + arr];
-            else if (d == a.ord) c = a.U[act * 3 + arr];
-          } else if (arr == 2) c = (ci == 5) ? a.z : 0.0; /* 2D: cz = (0,0,0,0,0,z) */
-          else if (arr == 3 && a.use_yaw) c = (ci == 5) ? row[12] : (ci == 4 ? a.Uyaw[act] : 0.0);
-          v = byte_of(c, bb);
+            if (d < c.ord) x = row[d * 3 + arr];
+            else if (d == c.ord) x = c.U[act * 3 + arr];
+          } else if (arr == 2) x = (ci == 5) ? a.z : 0.0; /* 2D: cz = (0,0,0,0,0,z) */
+          else if (arr == 3 && c.use_yaw) x = (ci == 5) ? row[12] : (ci == 4 ? c.Uyaw[act] : 0.0);
+          v = byte_of(x, bb);
         }
       }
       po[b] = v;
@@ -374,6 +376,7 @@ struct mplb_planner {
   DevBuf<mplb_result> d_results;
   DevBuf<int> d_actions;
   DevBuf<double> d_segs;
+  DevBuf<MplbTrajCfg> d_tcfg; /* the serialiser's one-entry configuration table */
   DevBuf<long long> d_phase; /* diagnostics build only */
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
 
@@ -1795,15 +1798,29 @@ int mplb_serialize_trajectories_device(mplb_planner *p, const void *d_results, c
   if (n <= 0) return MPLB_OK;
   if (max_seg <= 0) return fail(MPLB_ERR_ARG, "max_seg must be > 0");
   if (p->dirty || !p->map) return fail(MPLB_ERR_STATE, "no batch has been planned with the current configuration");
-  const size_t fl = frame_id ? std::strlen(frame_id) : 0;
-  if (fl > 64) return fail(MPLB_ERR_ARG, "frame_id longer than 64 bytes");
+  if ((frame_id ? std::strlen(frame_id) : 0) > 64) return fail(MPLB_ERR_ARG, "frame_id longer than 64 bytes");
   if (mplb_internal_set_device(p->device)) return fail(MPLB_ERR_CUDA, "cannot select the planner's device");
   const DevCfg &c = p->cfg;
+  MplbTrajCfg t; /* the batch's one configuration */
+  std::memset(&t, 0, sizeof(t));
+  t.dim = c.dim; t.ord = c.ord; t.control = c.control; t.use_yaw = c.use_yaw; t.U = c.U; t.Uyaw = c.Uyaw; t.dt = c.dt;
+  MPLB_CUDA_TRY(p->d_tcfg.reserve(1));
+  MPLB_CUDA_TRY(cudaMemcpyAsync(p->d_tcfg.p, &t, sizeof(t), cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  return mplb_internal_serialize(p->d_tcfg.p, nullptr, d_results, d_actions, d_seg_states, n, max_seg, z, seq, stamp_sec, stamp_nsec,
+                                 frame_id, d_out, stride, d_len, stream);
+}
+
+}  // extern "C"
+
+int mplb_internal_serialize(const MplbTrajCfg *d_cfgs, const int *d_cfg_id, const void *d_results, const void *d_actions,
+                            const void *d_seg_states, int n, int max_seg, double z, uint32_t seq, uint32_t stamp_sec,
+                            uint32_t stamp_nsec, const char *frame_id, void *d_out, size_t stride, void *d_len, void *stream) {
+  const size_t fl = frame_id ? std::strlen(frame_id) : 0;
   MsgArgs a;
   std::memset(&a, 0, sizeof(a));
   a.results = (const mplb_result *)d_results; a.actions = (const int *)d_actions; a.segs = (const double *)d_seg_states;
-  a.n = n; a.max_seg = max_seg; a.dim = c.dim; a.ord = c.ord; a.use_yaw = c.use_yaw; a.U = c.U; a.Uyaw = c.Uyaw;
-  a.dt = c.dt; a.z = z; a.seq = seq; a.sec = stamp_sec; a.nsec = stamp_nsec; a.frame_len = (unsigned)fl;
+  a.n = n; a.max_seg = max_seg; a.cfgs = d_cfgs; a.cfg_id = d_cfg_id;
+  a.z = z; a.seq = seq; a.sec = stamp_sec; a.nsec = stamp_nsec; a.frame_len = (unsigned)fl;
   if (fl) std::memcpy(a.frame, frame_id, fl);
   a.out = (unsigned char *)d_out; a.stride = stride; a.len = (unsigned *)d_len;
   const long long warps = (long long)n * (max_seg + 1);
@@ -1814,6 +1831,8 @@ int mplb_serialize_trajectories_device(mplb_planner *p, const void *d_results, c
   MPLB_CUDA_TRY(cudaStreamSynchronize((cudaStream_t)stream));
   return MPLB_OK;
 }
+
+extern "C" {
 
 int mplb_serialize_trajectories(mplb_planner *p, const mplb_result *results, const int32_t *actions, const double *seg_states,
                                 int n, int max_seg, double z, uint32_t seq, uint32_t stamp_sec, uint32_t stamp_nsec,

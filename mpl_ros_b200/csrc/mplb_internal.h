@@ -100,6 +100,31 @@ MPLB_HIDDEN int mplb_internal_lpa_enabled(mplb_planner *p);
 MPLB_HIDDEN int mplb_internal_lpa_plan(mplb_planner *p, const mplb_waypoint *start, const mplb_waypoint *goal, mplb_result *out);
 MPLB_HIDDEN void mplb_internal_lpa_drop(mplb_planner *p);
 
+/* ---- trajectory output of planned batches (the wire serialiser of mplb.cu, the waypoint gather of mplb_trajsolve.cu): what a
+ * plan's rows are read with.  Entry i of a batch uses table[cfg_id[i]] (cfg_id NULL: entry 0 for all).  An A* batch passes a table
+ * of one entry and no ids; an LPA* fleet passes one entry per planner (each session keeps its controls in its own device array)
+ * and ids 0 .. n-1. */
+struct MplbTrajCfg {
+  int dim, ord;      /* ord: 1 VEL .. 4 SNP, the control order the plan was made with */
+  int control;       /* the plan's Control flags (yaw bit included) */
+  int use_yaw;       /* the serialiser writes cyaw rows */
+  const double *U;   /* device, nU rows of 3 */
+  const double *Uyaw; /* device, nU yaw rates, or NULL */
+  double dt;
+};
+/* k_serialize_traj over n plans of the fixed-row layout (max_seg rows per plan) on `stream`; returns after it completed */
+MPLB_HIDDEN int mplb_internal_serialize(const MplbTrajCfg *d_cfgs, const int *d_cfg_id, const void *d_results, const void *d_actions,
+                                        const void *d_seg_states, int n, int max_seg, double z, uint32_t seq, uint32_t stamp_sec,
+                                        uint32_t stamp_nsec, const char *frame_id, void *d_out, size_t stride, void *d_len, void *stream);
+/* Trajectory::getWaypoints()[pick[i]] of every plan (t the running sum of segment times), ok[i] = 0 where there is none; enqueued */
+MPLB_HIDDEN int mplb_internal_pick_waypoints(const MplbTrajCfg *d_cfgs, const int *d_cfg_id, const void *d_results, const void *d_actions,
+                                             const void *d_seg_states, int n, int max_seg, const void *d_pick, void *d_wps, void *d_ok,
+                                             void *stream);
+/* the refinement of mplb_refine_trajectories_device for one dim, each plan with its own table entry; returns after the solve */
+MPLB_HIDDEN int mplb_internal_refine(int dim, const MplbTrajCfg *d_cfgs, const int *d_cfg_id, const void *d_results, const void *d_actions,
+                                     const void *d_seg_states, int n, int max_seg, int control, int yaw_control, void *d_coefs,
+                                     int32_t *n_segs, void *stream);
+
 /* ---- what the VoxelGrid unit (mplb_voxel.cu) needs from the map object of mplb.cu */
 struct mplb_map;
 struct MplbMapView {

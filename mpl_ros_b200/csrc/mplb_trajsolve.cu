@@ -34,6 +34,7 @@
 
 #include <algorithm>
 #include <cmath>
+#include <cstring>
 #include <string>
 #include <vector>
 
@@ -436,43 +437,109 @@ int ts_launch(int dim, int control, int yaw_control, int n_traj, const int32_t *
  * waypoint j < n_seg = the stored coord of segment j's parent (Primitive::evaluate(0) returns the coefficients c5, c4, c3, c2
  * = that state exactly), waypoint n_seg = the last primitive evaluated at its duration (pr:321-331 in the reference's term
  * order, mplb_ref.h); the two ends keep the plan's control flags, the interior ones become Control::VEL (map_planner_node.cpp:217-219).
- * One thread per (plan, waypoint); plan i owns slots [i * (max_seg + 1), ...). */
-__global__ void k_gather_waypoints(const mplb_result *res, const int *actions, const double *segs, int n, int max_seg, int dim,
-                                   int plan_control, const double *U, const double *Uyaw, double dt, mplb_waypoint *wps, double *dts) {
-  const int per = max_seg + 1;
+ * Plan i is read with cfgs[cfg_id ? cfg_id[i] : 0].
+ * pick == NULL: one thread per (plan, waypoint), plan i owns slots [i * (max_seg + 1), ...) of wps and [i * max_seg, ...) of dts,
+ *   t = j dt (the solver reads only the dts).
+ * pick != NULL: one thread per plan, the single waypoint pick[i] into wps[i] with the plan's control flags and t the running sum
+ *   0 + dt + ... + dt of getWaypoints (the next start of map_replanner_node.cpp:243-253); ok[i] = 0 and wps[i] untouched where the
+ *   plan failed, was truncated (n_seg > max_seg) or has no waypoint pick[i]. */
+__global__ void k_gather_waypoints(const mplb_result *res, const int *actions, const double *segs, int n, int max_seg,
+                                   const MplbTrajCfg *cfgs, const int *cfg_id, const int *pick, mplb_waypoint *wps, double *dts, int *ok) {
+  const int per = pick ? 1 : max_seg + 1;
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (long long)n * per) return;
-  const int i = (int)(idx / per), j = (int)(idx % per);
+  const int i = (int)(idx / per);
+  const int j = pick ? pick[i] : (int)(idx % per);
   const int ns = res[i].n_seg;
-  if (res[i].status != MPLB_PLAN_OK || ns < 1 || ns > max_seg || j > ns) return;
+  const bool have = res[i].status == MPLB_PLAN_OK && ns >= 1 && ns <= max_seg && j >= 0 && j <= ns;
+  if (pick) ok[i] = have ? 1 : 0;
+  if (!have) return;
+  const MplbTrajCfg c = cfgs[cfg_id ? cfg_id[i] : 0];
+  const int dim = c.dim, plan_control = c.control;
+  const double dt = c.dt;
   mplb_waypoint w;
   memset(&w, 0, sizeof(w));
-  const int cc = plan_control & 15;
-  const int ord = cc == 1 ? 1 : cc == 3 ? 2 : cc == 7 ? 3 : 4;
   if (j < ns) {
     const double *st = segs + ((size_t)i * max_seg + j) * 13;
     for (int k = 0; k < 3; k++) { w.pos[k] = st[k]; w.vel[k] = st[3 + k]; w.acc[k] = st[6 + k]; w.jrk[k] = st[9 + k]; }
     w.yaw = st[12];
-    dts[(size_t)i * max_seg + j] = dt;
+    if (!pick) dts[(size_t)i * max_seg + j] = dt;
   } else {
     const double *st = segs + ((size_t)i * max_seg + ns - 1) * 13;
     const int a = actions[(size_t)i * max_seg + ns - 1];
     mplb_ref::Prim pr;
     double e[13];
-    mplb_ref::prim_build(dim, ord, st, U + a * 3, pr);
+    mplb_ref::prim_build(dim, c.ord, st, c.U + a * 3, pr);
     mplb_ref::prim_eval(dim, pr, dt, e);
     for (int k = 0; k < dim; k++) { w.pos[k] = e[k]; w.vel[k] = e[3 + k]; w.acc[k] = e[6 + k]; w.jrk[k] = e[9 + k]; }
-    if ((plan_control & 16) && Uyaw) /* pr_yaw_.p(t) = c4 t + c5 with the zero terms in front, then normalize_angle */
-      w.yaw = mplb_ref::normalize_angle(mplb_ref::dadd(mplb_ref::dmul(Uyaw[a], dt), st[12]));
+    if ((plan_control & 16) && c.Uyaw) /* pr_yaw_.p(t) = c4 t + c5 with the zero terms in front, then normalize_angle */
+      w.yaw = mplb_ref::normalize_angle(mplb_ref::dadd(mplb_ref::dmul(c.Uyaw[a], dt), st[12]));
   }
-  w.t = __dmul_rn((double)j, dt);
-  w.control = (j == 0 || j == ns) ? plan_control : MPLB_CONTROL_VEL;
-  wps[(size_t)i * per + j] = w;
+  if (pick) {
+    double t = 0.0; /* trajectory.h:280-287 */
+    for (int m = 0; m < j; m++) t = __dadd_rn(t, dt);
+    w.t = t;
+    w.control = plan_control;
+    wps[i] = w;
+  } else {
+    w.t = __dmul_rn((double)j, dt);
+    w.control = (j == 0 || j == ns) ? plan_control : MPLB_CONTROL_VEL;
+    wps[(size_t)i * per + j] = w;
+  }
 }
+
+/* the gather of every waypoint, then one solve over the plans that are complete in the rows */
+int refine_run(int dim, const MplbTrajCfg *d_cfgs, const int *d_cfg_id, const mplb_result *d_res, const int *d_acts, const double *d_segs,
+               int n, int max_seg, int control, int yaw_control, double *d_coefs, int32_t *n_segs, cudaStream_t stream);
 
 thread_local TsScratch g_pwps, g_pdts, g_pU, g_pres;
 
+int refine_run(int dim, const MplbTrajCfg *d_cfgs, const int *d_cfg_id, const mplb_result *d_res, const int *d_acts, const double *d_segs,
+               int n, int max_seg, int control, int yaw_control, double *d_coefs, int32_t *n_segs, cudaStream_t stream) {
+  int Np = 0, Rp = 0, Ny = 0, Ry = 0;
+  const bool ok = ts_orders(control, &Np, &Rp) && (yaw_control == 1 || yaw_control == 3 || yaw_control == 7) && ts_orders(yaw_control, &Ny, &Ry);
+  std::vector<mplb_result> res(n);
+  MPLB_CUDA_TRY(cudaMemcpyAsync(res.data(), d_res, (size_t)n * sizeof(mplb_result), cudaMemcpyDeviceToHost, stream));
+  MPLB_CUDA_TRY(cudaStreamSynchronize(stream));
+  const int per = max_seg + 1;
+  std::vector<TsJob> jobs;
+  for (int i = 0; i < n; i++) {
+    const bool good = ok && res[i].status == MPLB_PLAN_OK && res[i].n_seg >= 1 && res[i].n_seg <= max_seg;
+    if (n_segs) n_segs[i] = good ? res[i].n_seg : 0;
+    if (!good) continue;
+    TsJob j;
+    j.wp_off = i * per; j.n_wp = res[i].n_seg + 1; j.seg_off = i * max_seg; j.pad = 0; j.ws_off = 0;
+    jobs.push_back(j);
+  }
+  MPLB_CUDA_TRY(g_pwps.reserve((size_t)n * per * sizeof(mplb_waypoint)));
+  MPLB_CUDA_TRY(g_pdts.reserve((size_t)n * max_seg * sizeof(double)));
+  MPLB_CUDA_TRY(cudaMemsetAsync(d_coefs, 0, (size_t)n * max_seg * (dim + 1) * 6 * sizeof(double), stream));
+  const long long total = (long long)n * per;
+  k_gather_waypoints<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(d_res, d_acts, d_segs, n, max_seg, d_cfgs, d_cfg_id, nullptr,
+                                                                           (mplb_waypoint *)g_pwps.p, (double *)g_pdts.p, nullptr);
+  mplb_internal_count_launches(1);
+  MPLB_CUDA_TRY(cudaGetLastError());
+  return ts_run(dim, Np, Rp, Ny, Ry, yaw_control, jobs, (const mplb_waypoint *)g_pwps.p, (const double *)g_pdts.p, d_coefs, stream);
+}
+
 }  // namespace
+
+int mplb_internal_refine(int dim, const MplbTrajCfg *d_cfgs, const int *d_cfg_id, const void *d_results, const void *d_actions,
+                         const void *d_seg_states, int n, int max_seg, int control, int yaw_control, void *d_coefs, int32_t *n_segs,
+                         void *stream) {
+  return refine_run(dim, d_cfgs, d_cfg_id, (const mplb_result *)d_results, (const int *)d_actions, (const double *)d_seg_states, n,
+                    max_seg, control, yaw_control, (double *)d_coefs, n_segs, (cudaStream_t)stream);
+}
+
+int mplb_internal_pick_waypoints(const MplbTrajCfg *d_cfgs, const int *d_cfg_id, const void *d_results, const void *d_actions,
+                                 const void *d_seg_states, int n, int max_seg, const void *d_pick, void *d_wps, void *d_ok, void *stream) {
+  k_gather_waypoints<<<(unsigned)((n + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
+      (const mplb_result *)d_results, (const int *)d_actions, (const double *)d_seg_states, n, max_seg, d_cfgs, d_cfg_id,
+      (const int *)d_pick, (mplb_waypoint *)d_wps, nullptr, (int *)d_ok);
+  mplb_internal_count_launches(1);
+  MPLB_CUDA_TRY(cudaGetLastError());
+  return MPLB_OK;
+}
 
 extern "C" {
 
@@ -503,39 +570,24 @@ int mplb_refine_trajectories_device(mplb_planner *p, const void *d_results, cons
   mplb_internal_planner_cfg(p, &hc);
   if (hc.nU <= 0) return mplb_internal_fail(MPLB_ERR_STATE, "refine: no controls set");
   MPLB_CUDA_TRY(cudaSetDevice(hc.device));
-  int Np = 0, Rp = 0, Ny = 0, Ry = 0;
-  const bool ok = ts_orders(control, &Np, &Rp) && (yaw_control == 1 || yaw_control == 3 || yaw_control == 7) && ts_orders(yaw_control, &Ny, &Ry);
-  std::vector<mplb_result> res(n);
-  MPLB_CUDA_TRY(cudaMemcpyAsync(res.data(), d_results, (size_t)n * sizeof(mplb_result), cudaMemcpyDeviceToHost, stream));
-  MPLB_CUDA_TRY(cudaStreamSynchronize(stream));
-  const int per = max_seg + 1;
-  std::vector<TsJob> jobs;
-  for (int i = 0; i < n; i++) {
-    const bool good = ok && res[i].status == MPLB_PLAN_OK && res[i].n_seg >= 1 && res[i].n_seg <= max_seg;
-    if (n_segs) n_segs[i] = good ? res[i].n_seg : 0;
-    if (!good) continue;
-    TsJob j;
-    j.wp_off = i * per; j.n_wp = res[i].n_seg + 1; j.seg_off = i * max_seg; j.pad = 0; j.ws_off = 0;
-    jobs.push_back(j);
-  }
-  MPLB_CUDA_TRY(g_pwps.reserve((size_t)n * per * sizeof(mplb_waypoint)));
-  MPLB_CUDA_TRY(g_pdts.reserve((size_t)n * max_seg * sizeof(double)));
-  MPLB_CUDA_TRY(g_pU.reserve((size_t)hc.nU * 4 * sizeof(double)));
-  MPLB_CUDA_TRY(cudaMemcpyAsync(g_pU.p, hc.U, (size_t)hc.nU * 3 * sizeof(double), cudaMemcpyHostToDevice, stream));
+  /* the batch's one configuration: the planner's controls and dt, the control flags it was planned with */
+  MPLB_CUDA_TRY(g_pU.reserve((size_t)hc.nU * 4 * sizeof(double) + sizeof(MplbTrajCfg)));
+  MplbTrajCfg *d_cfg = (MplbTrajCfg *)g_pU.p;
+  double *d_U = (double *)(g_pU.p + sizeof(MplbTrajCfg));
+  MPLB_CUDA_TRY(cudaMemcpyAsync(d_U, hc.U, (size_t)hc.nU * 3 * sizeof(double), cudaMemcpyHostToDevice, stream));
   double *d_Uyaw = nullptr;
   if (hc.Uyaw) {
-    d_Uyaw = (double *)g_pU.p + (size_t)hc.nU * 3;
+    d_Uyaw = d_U + (size_t)hc.nU * 3;
     MPLB_CUDA_TRY(cudaMemcpyAsync(d_Uyaw, hc.Uyaw, (size_t)hc.nU * sizeof(double), cudaMemcpyHostToDevice, stream));
   }
-  MPLB_CUDA_TRY(cudaMemsetAsync(d_coefs, 0, (size_t)n * max_seg * (hc.dim + 1) * 6 * sizeof(double), stream));
-  const long long total = (long long)n * per;
-  k_gather_waypoints<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>((const mplb_result *)d_results, (const int *)d_actions,
-                                                                           (const double *)d_seg_states, n, max_seg, hc.dim, plan_control,
-                                                                           (const double *)g_pU.p, d_Uyaw, hc.dt, (mplb_waypoint *)g_pwps.p,
-                                                                           (double *)g_pdts.p);
-  mplb_internal_count_launches(1);
-  MPLB_CUDA_TRY(cudaGetLastError());
-  return ts_run(hc.dim, Np, Rp, Ny, Ry, yaw_control, jobs, (const mplb_waypoint *)g_pwps.p, (const double *)g_pdts.p, (double *)d_coefs, stream);
+  const int cc = plan_control & 15;
+  MplbTrajCfg t;
+  std::memset(&t, 0, sizeof(t));
+  t.dim = hc.dim; t.ord = cc == 1 ? 1 : cc == 3 ? 2 : cc == 7 ? 3 : 4; t.control = plan_control; t.use_yaw = (plan_control & 16) ? 1 : 0;
+  t.U = d_U; t.Uyaw = d_Uyaw; t.dt = hc.dt;
+  MPLB_CUDA_TRY(cudaMemcpyAsync(d_cfg, &t, sizeof(t), cudaMemcpyHostToDevice, stream));
+  return refine_run(hc.dim, d_cfg, nullptr, (const mplb_result *)d_results, (const int *)d_actions, (const double *)d_seg_states, n,
+                    max_seg, control, yaw_control, (double *)d_coefs, n_segs, stream);
 }
 
 int mplb_refine_trajectories(mplb_planner *p, const mplb_result *results, const int32_t *actions, const double *seg_states, int n,

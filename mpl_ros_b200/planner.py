@@ -527,6 +527,60 @@ class MapPlanner:
         check(lib().mplb_lpa_plan_batch(MapPlanner._handles(planners), n, ptr(s), ptr(g), ptr(res)))
         return [pl._planned(res[i], int(s["control"][i])) for i, pl in enumerate(planners)]
 
+    # ---- a fleet cycle's output on the device.  Buffers are torch CUDA tensors or device addresses (ints); `stream` a
+    # torch.cuda.Stream, a cudaStream_t as int, or None for the default stream.  Every call returns after its work completed.
+    @staticmethod
+    def _dev(x):
+        if x is None:
+            return None
+        if hasattr(x, "data_ptr"):
+            return C.c_void_p(x.data_ptr())
+        if hasattr(x, "cuda_stream"):
+            return C.c_void_p(x.cuda_stream) if x.cuda_stream else None
+        return C.c_void_p(int(x)) if int(x) else None
+
+    @staticmethod
+    def planLPABatchDevice(planners, d_starts, d_goals, d_results, d_actions=None, d_segs=None, max_seg=0, stream=None):
+        """mplb_lpa_plan_batch_device: planLPABatch with device starts / goals [n] (waypoint records) and results [n]; plan i's
+        first max_seg action ids and seg-state rows go to d_actions[i] / d_segs[i] (mplb_plan_batch_device's layout).  Nothing
+        is read back: the library keeps each planner's trajectory for getActions / getSegStates, while the Python-side
+        result(), traj_ and traj_cost_ are left as they were."""
+        d = MapPlanner._dev
+        check(lib().mplb_lpa_plan_batch_device(MapPlanner._handles(planners), len(planners), d(d_starts), d(d_goals), d(d_results),
+                                               d(d_actions), d(d_segs), int(max_seg), d(stream)))
+
+    @staticmethod
+    def trajectoryWaypointsBatch(planners, d_results, d_actions, d_segs, max_seg, d_index, d_waypoints, d_ok, stream=None):
+        """mplb_lpa_trajectory_waypoints_device: d_waypoints[i] = getTraj().getWaypoints()[d_index[i]] of plan i of the
+        plan-batch layout (t the running sum of segment times), d_ok[i] = 0 where plan i has no such waypoint.  The output can
+        be the next cycle's d_starts (map_replanner_node.cpp:243-253)."""
+        d = MapPlanner._dev
+        check(lib().mplb_lpa_trajectory_waypoints_device(MapPlanner._handles(planners), len(planners), d(d_results), d(d_actions),
+                                                         d(d_segs), int(max_seg), d(d_index), d(d_waypoints), d(d_ok), d(stream)))
+
+    @staticmethod
+    def serializeLPABatch(planners, d_results, d_actions, d_segs, max_seg, d_out, stride, d_len, z=0.0, frame_id="map", seq=0,
+                          stamp=(0, 0), stream=None):
+        """mplb_lpa_serialize_trajectories_device: the planning_ros_msgs/Trajectory wire bytes of every plan of the
+        plan-batch layout, plan i with planner i's own controls and dt, to d_out + i * stride; byte counts to d_len (uint32)."""
+        d = MapPlanner._dev
+        check(lib().mplb_lpa_serialize_trajectories_device(MapPlanner._handles(planners), len(planners), d(d_results), d(d_actions),
+                                                           d(d_segs), int(max_seg), float(z), int(seq), int(stamp[0]), int(stamp[1]),
+                                                           frame_id.encode(), d(d_out), int(stride), d(d_len), d(stream)))
+
+    @staticmethod
+    def refineLPABatch(planners, d_results, d_actions, d_segs, max_seg, d_coefs, control=JRK, yaw_control=VEL, stream=None):
+        """mplb_lpa_refine_trajectories_device: map_planner_node.cpp:216-227 for every plan of the plan-batch layout, plan i
+        with planner i's own controls, dt and control flags; coefficient rows to d_coefs [n, max_seg, dim + 1, 6] (float64).
+        Returns the refined segment counts."""
+        n = len(planners)
+        nseg = np.zeros(max(n, 1), dtype=np.int32)
+        d = MapPlanner._dev
+        check(lib().mplb_lpa_refine_trajectories_device(MapPlanner._handles(planners), n, d(d_results), d(d_actions), d(d_segs),
+                                                        int(max_seg), int(control), int(yaw_control), d(d_coefs), ptr(nseg),
+                                                        d(stream)))
+        return [int(v) for v in nseg[:n]]
+
     @staticmethod
     def planLPAFleet(comm, planners, n_total, starts, goals, max_seg=64, root=0):
         """mplb_fleet_plan: planLPABatch of this rank's robots (planners: robots rank, rank + N, ... of n_total, on comm's
